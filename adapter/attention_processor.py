@@ -1,6 +1,6 @@
 """Drop-in for the reference's `adapter/attention_processor.py`: same module path, class names, constructor
 signatures, parameter names (state_dict keys `to_k_ref.weight`, `to_k_ip.weight`, `to_q_lora.down.weight`, ...),
-mutable attributes (`scale`, `lora_scale`, `name`, `cache`) and call signature — executing on the sm_100a
+mutable attributes (`scale`, `lora_scale`, `name`, `cache`) and call signature — executing on the sm_90a
 kernels through imagdressing_b200.processors.attention_forward. See that module for how the arithmetic maps to
 kernels; every class cites the reference lines it replaces (relative to /root/reference).
 

@@ -1,7 +1,7 @@
 """Drop-in for the reference's `adapter/resampler.py`: `Resampler` (the garment `ImgProj`,
 inference_IMAGdressing.py:55-65) and `ProjPlusModel` (FaceID-Plus projector,
 IMAGDressing_v1_pipeline_ipa_controlnet.py:79-86) with the reference's constructor arguments and state_dict keys,
-executing on the sm_100a kernels: LayerNorm kernel, tcgen05 GEMMs (GELU / residual epilogues) and the same
+executing on the sm_90a kernels: LayerNorm kernel, wgmma GEMMs (GELU / residual epilogues) and the same
 attention kernel as the UNet (16 or 4 latent queries against 257 CLIP tokens + the latents, 64-wide heads;
 `(q d^-1/4)(k d^-1/4)^T` == `q k^T / sqrt(d)`, softmax statistics in fp32 — adapter/resampler.py:62-78).
 """

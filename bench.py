@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — images/sec of IMAGDressing-v1 garment-conditioned sampling (512x512, 50 DDIM steps, CFG) on B200.
+"""bench.py — images/sec of IMAGDressing-v1 garment-conditioned sampling (512x512, 50 DDIM steps, CFG) on H100.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--batch B] [--impl reference]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 bench.py --gpus N ...
@@ -25,6 +25,7 @@ import time
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
+import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
 HW = 64  # 512 / 8
@@ -48,6 +49,9 @@ def parse():
                     help="base = configs[1] (the metric); ipa_controlnet = configs[2]; inpaint = configs[3]")
     ap.add_argument("--height", type=int, default=512)
     ap.add_argument("--width", type=int, default=512)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the output latents of the last timed step to DIR/latents.npy (float32; above 64 MB a "
+                         "fixed sample, DIR/latents_sample.npy)")
     return ap.parse_args()
 
 
@@ -55,12 +59,12 @@ def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get("hbm_gbs", 6650.0), d.get("bf16_tflops", 1590.0), d.get("bf16_tflops_sustained", 1400.0), "measured"
-    return 6650.0, 1590.0, 1400.0, "fallback"
+        return d.get("hbm_gbs", 3350.0), d.get("bf16_tflops", 989.0), d.get("bf16_tflops_sustained", 989.0), "measured"
+    return 3350.0, 989.0, 989.0, "fallback"  # H100 SXM data sheet (HBM3, dense BF16)
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
 
     Q = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -313,9 +317,8 @@ def train_record(a, dev, rank, local, world, B, h, w, steps, warm):
 
 # ------------------------------------------------------------------------------------------------ roofline legs
 def ncu_traffic_table():
-    """DRAM bytes per launch (dram__bytes_read.sum + dram__bytes_write.sum) of the roofline kernels, extracted from the
-    committed `ncu --set full` captures by tools/ncu_summary.py into profiles/ncu_traffic.json ({kernel: {"bytes": ...,
-    "source": "<profiles/ file>"}}); a kernel without a capture reports null."""
+    """DRAM bytes per launch of the roofline kernels from profiles/ncu_traffic.json ({kernel: {"bytes": ..., "source":
+    ...}}) when such captures exist; a kernel without a capture reports null."""
     path = os.path.join(ROOT, "profiles", "ncu_traffic.json")
     try:
         return json.load(open(path))
@@ -331,7 +334,7 @@ def kernel_roofline(dev, B):
     from imagdressing_b200 import ops
 
     hbm, tf_burst, tf_sus, src = peaks()
-    flush = torch.empty(160 * 1024 * 1024, device=dev, dtype=torch.int32)  # 640 MB > 126 MB L2
+    flush = torch.empty(160 * 1024 * 1024, device=dev, dtype=torch.int32)  # 640 MB > 50 MB L2
 
     def timeit(fn, iters=10):
         fn()
@@ -540,8 +543,26 @@ def cpu_baseline(sample_forwards=CPU_SAMPLE_FORWARDS, threads=None):
 
 
 # ------------------------------------------------------------------------------------------------ main
+DUMP_MAX_BYTES = 64 << 20
+
+
+def dump_output(directory, name, t):
+    """directory/name.npy in float32. Above 64 MB a fixed sample is written instead: the elements at the sorted positions
+    of a seed-0 permutation of the flattened output, as many as fit."""
+    os.makedirs(directory, exist_ok=True)
+    out = t.detach().float().cpu()
+    keep = DUMP_MAX_BYTES // 4
+    if out.numel() > keep:
+        idx = torch.randperm(out.numel(), generator=torch.Generator().manual_seed(0))[:keep].sort().values
+        out, name = out.flatten()[idx], name + "_sample"
+    np.save(os.path.join(directory, name + ".npy"), out.numpy())
+
+
 def main():
     a = parse()
+    if a.dump_outputs and (a.impl == "reference" or a.workload == "train"):
+        raise SystemExit("bench.py: --dump-outputs covers the sampling workloads of the kernel path; "
+                         "--impl reference and --workload train have no output dump")
     rank = int(os.environ.get("RANK", "0"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -665,9 +686,16 @@ def main():
     if rank == 0:
         clk.start()
     l0 = _lib.launch_count
-    ms_total = timed(lambda: one_step(x_dev), a.steps)
+    last = {}
+
+    def timed_step():
+        last["latents"] = one_step(x_dev)
+
+    ms_total = timed(timed_step, a.steps)
     launches = _lib.launch_count - l0
     clocks = clk.stop() if rank == 0 else None
+    if a.dump_outputs and rank == 0:  # the inputs are seeded, so two builds can be compared output for output
+        dump_output(a.dump_outputs, "latents", last["latents"])
     one_step_e2e()
     ms_e2e = timed(one_step_e2e, a.steps)
 
@@ -758,7 +786,7 @@ def main():
                                "SD1.5 denoising UNet + garment UNet; timed region = garment pass + 50 steps "
                                "(VAE/CLIP excluded)",
                    "global_batch": world * B, "latent": [lh, lw], "ddim_steps": STEPS_DDIM, "parallelism": f"dp{world}",
-                   "l2": "activations+weights (3.4 GB bf16) exceed the 126 MB L2; no explicit flush between steps"},
+                   "l2": "activations+weights (3.4 GB bf16) exceed the 50 MB L2; no explicit flush between steps"},
         "e2e": {"value": round(e2e_v, 4), "unit": "images/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h},
         "gpu_launches": launches, "clocks": clocks,
         "roofline": roofline, "kernels": roofs,

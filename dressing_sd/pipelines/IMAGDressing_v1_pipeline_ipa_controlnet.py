@@ -1,6 +1,6 @@
 """Drop-in for the reference's dressing_sd/pipelines/IMAGDressing_v1_pipeline_ipa_controlnet.py: same import path and class name
 (`IMAGDressing_v1`), constructor and `__call__` keyword arguments; implemented by
-imagdressing_b200.pipelines.IMAGDressing_v1_IPAControlNet on the sm_100a kernels."""
+imagdressing_b200.pipelines.IMAGDressing_v1_IPAControlNet on the sm_90a kernels."""
 from imagdressing_b200.pipelines import IMAGDressing_v1_IPAControlNet as _Impl
 from imagdressing_b200.pipelines import StableDiffusionPipelineOutput  # noqa: F401
 

@@ -1,4 +1,4 @@
-"""imagdressing_b200 — B200-native (sm_100a) kernels + host mirror for the IMAGDressing-v1 denoising hot path.
+"""imagdressing_b200 — H100-native (sm_90a) kernels + host mirror for the IMAGDressing-v1 denoising hot path.
 
 Only what the path needs lives here: `csrc/` (CUDA kernels + the C ABI of include/imagd_b200.h), `_lib` / `ops`
 (ctypes binding), and the host-side mirror of the reference interfaces (UNet / ControlNet hosts, attention

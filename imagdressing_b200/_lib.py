@@ -1,7 +1,7 @@
 """ctypes binding of libimagd_b200.so (the C ABI declared in include/imagd_b200.h).
 
 The library is the product: there is no CPU or PyTorch fallback. Importing this module never needs a GPU (the
-build check and the symbol test run on a CPU box); calling a kernel without the library or without a B200 raises.
+build check and the symbol test run on a CPU box); calling a kernel without the library or without an H100 (sm_90) raises.
 """
 from __future__ import annotations
 
@@ -236,4 +236,4 @@ def require_b200() -> None:
     rc = load().imagd_device_check()
     if rc < 0:
         msg = load().imagd_last_error()
-        raise ImagdError(f"imagd_b200 needs an sm_100 GPU: {msg.decode() if msg else rc}")
+        raise ImagdError(f"imagd_b200 needs an sm_90 (H100) GPU: {msg.decode() if msg else rc}")

@@ -2,12 +2,12 @@
 under autograd, :573-605 loss + backward). torch autograd only ORDERS the backward pass and accumulates fan-out gradients;
 every forward and backward computation below is a kernel of libimagd_b200.so:
 
-  Linear      y = x W^T + b (+ residual)        dX = dY W            (tcgen05 GEMM on W^T)
-                                                dW = dY^T X          (tcgen05 GEMM on the two transposed operands, K = tokens)
+  Linear      y = x W^T + b (+ residual)        dX = dY W            (wgmma GEMM on W^T)
+                                                dW = dY^T X          (wgmma GEMM on the two transposed operands, K = tokens)
                                                 db = column sum of dY
-  Conv3x3     implicit-GEMM conv                dX = conv3x3(dY, flipped / transposed taps)    (the same tcgen05 conv kernel)
-                                                dW = dY^T im2col(X)^T (tcgen05 GEMM), db / d(time-embedding row) = column sums
-  Attention   two-stream flash forward          dQ / dK / dV / dK_ref / dV_ref: attention_bwd.cu (tcgen05, recompute-S)
+  Conv3x3     implicit-GEMM conv                dX = conv3x3(dY, flipped / transposed taps)    (the same wgmma conv kernel)
+                                                dW = dY^T im2col(X)^T (wgmma GEMM), db / d(time-embedding row) = column sums
+  Attention   two-stream flash forward          dQ / dK / dV / dK_ref / dV_ref: attention_bwd.cu (recompute-S)
   GroupNorm(+SiLU), LayerNorm, SiLU / GELU, GEGLU, nearest-2x upsample, stride-2 im2col, channel concat, MSE: train_ops.cu
 
 Activations are bf16 token-major exactly as on the inference path; gradients are bf16 (fp32 accumulation inside every kernel),

@@ -1,6 +1,6 @@
 """Checkpoint / weight-format loader for the IMAGDressing-v1 hot path (SURVEY.md §8f-2).
 
-Three on-disk formats reach the reference's models, all restated here so real weights can run on the sm_100a kernels:
+Three on-disk formats reach the reference's models, all restated here so real weights can run on the sm_90a kernels:
 
 1. The DeepSpeed training checkpoint `IMAGDressing-v1_512.pt`: `torch.load(path)["module"]` is the state_dict of
    `train.py`'s `SDModel` (members `unet`, `ref_unet`, `proj`, `adapter_modules`, train.py:244-253), routed by key

@@ -1,4 +1,4 @@
-"""CLIP text / vision encoders on the sm_100a kernels (SURVEY.md §8f row 3).
+"""CLIP text / vision encoders on the sm_90a kernels (SURVEY.md §8f row 3).
 
 The reference builds them with `transformers` (`CLIPTextModel`, `CLIPVisionModelWithProjection`,
 inference_IMAGdressing.py:44-49) and calls them at the edges of the path:
@@ -8,7 +8,7 @@ inference_IMAGdressing.py:44-49) and calls them at the edges of the path:
 
 Those modules stay the PARAMETER CONTAINERS (so `from_pretrained`, `.to()`, `state_dict()` and the checkpoints keep
 working unchanged); `accelerate(module)` wraps one in an executor that runs the forward on this library's kernels instead of
-torch / cuBLAS: token + position embedding gather, patch embedding as a tcgen05 GEMM over patch rows, pre-LN transformer
+torch / cuBLAS: token + position embedding gather, patch embedding as a wgmma GEMM over patch rows, pre-LN transformer
 layers = LayerNorm kernel -> fused QKV GEMM (+bias) -> the attention kernel (causal for text; head_dim 64 text / 80 ViT-H)
 -> out-projection GEMM with bias + residual in the epilogue -> LayerNorm -> fc1 GEMM with bias + (quick_)GELU in the
 epilogue -> fc2 GEMM with bias + residual. The pipelines wrap CUDA-resident CLIP modules automatically (IMAGD_CLIP_KERNELS=0

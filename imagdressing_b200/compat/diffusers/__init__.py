@@ -3,8 +3,8 @@ the callers"): put `imagdressing_b200/compat` on PYTHONPATH *instead of* a diffu
 
     from diffusers import UNet2DConditionModel, AutoencoderKL, DDIMScheduler, ControlNetModel
 
-resolves to the B200 host models of this repo: the denoising / garment UNet, the ControlNet, the DDIM scheduler and (round 2,
-SURVEY.md §8f row 1) the VAE, all executing on the sm_100a kernels.
+resolves to the H100 host models of this repo: the denoising / garment UNet, the ControlNet, the DDIM scheduler and (round 2,
+SURVEY.md §8f row 1) the VAE, all executing on the sm_90a kernels.
 Never shadow a real diffusers install with this package by accident: it is not on the path unless you add it.
 """
 from imagdressing_b200.modeling import ControlNetModel, UNet2DConditionModel  # noqa: F401

@@ -16,8 +16,8 @@ void set_error(const char* fmt, ...) {
     va_end(ap);
 }
 
-// IMAGD_PDL: 0 (default) no programmatic dependent launch; 1 every kernel lets its dependent start at once (round 1:
-// neutral-to-negative on the B=1 step - the dependent's CTAs take shared memory / TMEM the running kernel still needs);
+// IMAGD_PDL: 0 (default) no programmatic dependent launch; 1 every kernel lets its dependent start at once (the
+// dependent's CTAs can take shared memory the running kernel still needs);
 // 2 "late trigger": the tensor-core kernels release their dependent only when their own mainloop is done, so the next
 // kernel's launch latency and prologue hide under this kernel's epilogue / tail instead of competing with its mainloop.
 int pdl_mode() {
@@ -107,8 +107,8 @@ int imagd_device_check(void) {
     cudaDeviceProp p;
     e = cudaGetDeviceProperties(&p, dev);
     if (e != cudaSuccess) return imagd::cuda_fail(e, "cudaGetDeviceProperties");
-    if (p.major != 10) {
-        imagd::set_error("device %s is sm_%d%d; this library is built for sm_100a only", p.name, p.major, p.minor);
+    if (p.major != 9 || p.minor != 0) {
+        imagd::set_error("device %s is sm_%d%d; this library is built for sm_90a only", p.name, p.major, p.minor);
         return IMAGD_ERR_ARCH;
     }
     return p.major * 10 + p.minor;

@@ -1,4 +1,4 @@
-// Backward of the two-stream ("hybrid") attention on tcgen05 for sm_100a — the training step of SURVEY.md section 8 row
+// Backward of the two-stream ("hybrid") attention for sm_90a — the training step of SURVEY.md section 8 row
 // a13 (reference train.py:255-281,573-605: loss -> frozen denoising UNet -> to_k_ref / to_v_ref and the garment taps ->
 // garment UNet; the reference gets this from torch autograd over F.scaled_dot_product_attention,
 // adapter/attention_processor.py:589-612).
@@ -7,22 +7,14 @@
 //   per stream:  P = exp2(S s log2e - lse2),  dP = w dO V^T,  D = rowsum(P o dP) = w rowsum(dO o O_s),
 //                dS = P o (dP - D),  dQ += s dS K,  dK = s dS^T Q,  dV = w P^T dO
 //
-// Recompute-S flash style, two kernels, no atomics, deterministic:
-//   * attn_bwd_dq_kernel   one CTA per 128 queries of a (sample, head); K/V blocks of both streams stream through a TMA
-//                          ring; S = Q K^T and dP = dO V^T land in TMEM, 8 warps turn them into dS (bf16, swizzled smem),
-//                          dQ += dS K accumulates in TMEM over BOTH streams.
-//   * attn_bwd_dkv_kernel  one CTA per 128 keys of a (sample, head) of ONE stream; Q / dO blocks stream through the ring;
-//                          the TRANSPOSED products S^T = K Q^T and dP^T = V dO^T land in TMEM (lane = key), so P^T and
-//                          dS^T are written row-major by their owning threads and dV += P^T dO, dK += dS^T Q need no
-//                          transposes anywhere: the Q / dO tiles that fed the first two products K-major are read again
-//                          MN-major (the same shared-memory bytes, another descriptor) — as V is in the forward's P.V.
-// Operand forms are exactly the forward kernel's (K-major A and B for the score products, K-major A from swizzled smem +
-// MN-major B for the second products), so the descriptors are the validated ones.
+// Recompute-S flash style, two kernels, no atomics, deterministic (attn_bwd_dq_kernel: dQ over both streams;
+// attn_bwd_dkv_kernel: dK / dV of one stream), on mma.sync m16n8k16 tensor-core tiles fed from padded shared memory.
 // lse2 / D rows arrive as fp32 vectors [2 streams][B][heads][lq_pad]; lse2 of padding rows is +inf (P = 0).
 #include <cstdlib>
 
 #include "common.cuh"
 #include "ptx.cuh"
+#include "attention_common.cuh"
 
 namespace imagd {
 
@@ -30,7 +22,11 @@ struct AttnBwdParams {
     int B, Lq, heads, hd;
     float scale_log2;  // sm_scale * log2(e)
     float sm_scale;
-    int len0, len1;  // keys per sample of stream 0 / 1 (len1 = 0: one stream)
+    const __nv_bfloat16* q;
+    int64_t q_ld;
+    const __nv_bfloat16* d_out;
+    int64_t do_ld;
+    AttnKV kv[2];    // kv[1].len = 0: one stream
     float w0, w1;    // out_scale of the streams
     int lq_pad;
     const float* lse;   // [2][B][heads][lq_pad]
@@ -44,570 +40,224 @@ struct AttnBwdParams {
     void* dv;
     int64_t dkv_ld;
     int kv_sample_rows;  // rows between samples in dk / dv
-    int spin;            // 1: the dS / P warps spin on their mbarriers instead of suspending (IMAGD_BWD_SPIN, A/B)
 };
-
-__device__ __forceinline__ void bwd_wait(uint64_t* bar, uint32_t parity, int spin) {
-    if (spin) mbar_wait_spin(bar, parity);
-    else mbar_wait(bar, parity);
-}
-
-constexpr int kBAtom = 128 * 128;  // one [128 rows x 64 bf16] swizzled tile
-
-// fp32 pair -> bf16x2. PACK = 0: cvt.rn.bf16x2.f32 (F2FP, on the XU pipe next to MUFU.EX2); PACK = 2: add half an ulp to the
-// bit patterns, then ONE byte permute picks the two high halves (round-half-up of the magnitude; ALU pipe only). Runtime A/B
-// for the head-dim-40 kernels through IMAGD_BWD_PACK.
-template <int PACK>
-__device__ __forceinline__ uint32_t bwd_pack(float lo, float hi) {
-    if constexpr (PACK == 0) {
-        return pack_bf16x2(lo, hi);
-    } else {
-        return __byte_perm(__float_as_uint(lo) + 0x8000u, __float_as_uint(hi) + 0x8000u, 0x7632);
-    }
-}
 
 // ------------------------------------------------------------------------------------------------ dQ kernel
-template <int HD_MMA, int NATOM, int KV_STAGES, int DSB = 1>
-struct DqCfg {
-    static constexpr int kQOff = 0;
-    static constexpr int kDoOff = NATOM * kBAtom;
-    static constexpr int kKOff = 2 * NATOM * kBAtom;
-    static constexpr int kVOff = kKOff + KV_STAGES * NATOM * kBAtom;
-    static constexpr int kDsOff = kVOff + KV_STAGES * NATOM * kBAtom;
-    static constexpr int kBarOff = kDsOff + DSB * 2 * kBAtom;  // DSB dS buffers of two atoms
-    static constexpr int kNumBars = 1 + 2 * KV_STAGES + 3 + 2 * DSB;  // q, kv_full / kv_empty per stage, s_full, o_full, s_free, p_full[DSB], pv_done[DSB]
-    static constexpr int kTotal = kBarOff + kNumBars * 8 + 16;
-    static_assert(kTotal <= 232448, "dq kernel: shared memory");
-    static_assert(256 + HD_MMA <= 512, "dq kernel: TMEM");
+// CTA = 128 queries of one (sample, head), 8 warps of 16 rows; K / V blocks of 64 keys of both streams stream through
+// a two-stage ring. Per block: S = Q K^T and dP = dO V^T (mma.sync), P = exp2(S s log2e - lse2), dS = P o (w dP - D),
+// dQ += dS K with dS kept in registers as the A fragment.
+template <int HDP>
+struct BwdDqSmem {
+    static constexpr int kQBytes = 128 * attn_row_bytes(HDP);
+    static constexpr int kKVBytes = 64 * attn_row_bytes(HDP);
+    static constexpr int kDoOff = kQBytes;
+    static constexpr int kKOff = 2 * kQBytes;
+    static constexpr int kVOff = kKOff + 2 * kKVBytes;
+    static constexpr int kTotal = kVOff + 2 * kKVBytes;
 };
 
-// DSB = 2: dS is double-buffered (with its own p_full / pv_done barrier pair per buffer), so the exponentials and stores of key
-// block i+1 run while the tensor core still reads dS(i) for dQ += dS K — with one buffer every block serialises
-// softmax -> dQ MMA -> softmax (measured ~3200 clk per block against 1024 clk of exponentials).
-template <int HD_MMA, int NATOM, int KV_STAGES, int PACK = 0, int DSB = 1>
-__global__ void __launch_bounds__(320, 1)
-attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmDO,
-                   const __grid_constant__ CUtensorMap tmK0, const __grid_constant__ CUtensorMap tmV0,
-                   const __grid_constant__ CUtensorMap tmK1, const __grid_constant__ CUtensorMap tmV1,
-                   const AttnBwdParams p) {
-    using C = DqCfg<HD_MMA, NATOM, KV_STAGES, DSB>;
-    extern __shared__ __align__(1024) uint8_t smem[];
-    if (threadIdx.x == 0 && (smem_u32(smem) & 1023u) != 0) __trap();
-    uint8_t* sQ = smem + C::kQOff;
-    uint8_t* sDO = smem + C::kDoOff;
-    uint8_t* sK = smem + C::kKOff;
-    uint8_t* sV = smem + C::kVOff;
-    uint8_t* sDS = smem + C::kDsOff;
-    uint64_t* q_full = reinterpret_cast<uint64_t*>(smem + C::kBarOff);
-    uint64_t* kv_full = q_full + 1;
-    uint64_t* kv_empty = kv_full + KV_STAGES;
-    uint64_t* s_full = kv_empty + KV_STAGES;
-    uint64_t* o_full = s_full + 1;
-    uint64_t* s_free = o_full + 1;
-    uint64_t* p_full = s_free + 1;       // [DSB]
-    uint64_t* pv_done = p_full + DSB;    // [DSB]
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(pv_done + DSB);
+// 16 x 64 product of a 16-row A tile (rows arow.. of sA) and 64 B rows (brow.. of sB), K = HDP, both row-major in smem
+template <int HDP>
+__device__ __forceinline__ void bwd_mma_abt(float (&c)[8][4], uint32_t sA, int arow, uint32_t sB, int lane) {
+    constexpr int kRow = attn_row_bytes(HDP);
+#pragma unroll
+    for (int n = 0; n < 8; ++n) c[n][0] = c[n][1] = c[n][2] = c[n][3] = 0.f;
+#pragma unroll
+    for (int ks = 0; ks < HDP / 16; ++ks) {
+        uint32_t a[4];
+        ldmatrix_x4(a, sA + (arow + (lane & 15)) * kRow + (ks * 16 + (lane >> 4) * 8) * 2);
+#pragma unroll
+        for (int np = 0; np < 4; ++np) {
+            uint32_t bb[4];
+            ldmatrix_x4(bb, sB + (np * 16 + (lane & 7) + (lane >> 4) * 8) * kRow + (ks * 16 + ((lane >> 3) & 1) * 8) * 2);
+            mma_bf16_16816(c[2 * np], a, bb[0], bb[1]);
+            mma_bf16_16816(c[2 * np + 1], a, bb[2], bb[3]);
+        }
+    }
+}
 
-    const int warp = threadIdx.x >> 5;
-    const int q0 = blockIdx.x * 128;
-    const int h = blockIdx.y;
-    const int b = blockIdx.z;
-    const int nb0 = (p.len0 + 127) / 128;
-    const int nb1 = (p.len1 + 127) / 128;
+// acc[16 x HDP] += A[16 x 64] (bf16 fragments a[kk], kk = 16-column step) * B[64 x HDP] (rows of sB, row-major in smem)
+template <int HDP>
+__device__ __forceinline__ void bwd_mma_ab(float (&acc)[HDP / 8][4], const uint32_t (&a)[4][4], uint32_t sB, int lane) {
+    constexpr int kRow = attn_row_bytes(HDP);
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+#pragma unroll
+        for (int np = 0; np < HDP / 16; ++np) {
+            uint32_t bb[4];
+            ldmatrix_x4_trans(bb, sB + (kk * 16 + (lane & 7) + ((lane >> 3) & 1) * 8) * kRow + (np * 16 + (lane >> 4) * 8) * 2);
+            mma_bf16_16816(acc[2 * np], a[kk], bb[0], bb[1]);
+            mma_bf16_16816(acc[2 * np + 1], a[kk], bb[2], bb[3]);
+        }
+    }
+}
+
+// C fragments of a 16 x 64 tile -> bf16 A fragments of the same tile
+__device__ __forceinline__ void bwd_pack_a(const float (&c)[8][4], uint32_t (&a)[4][4]) {
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+        a[kk][0] = pack_bf16x2(c[2 * kk][0], c[2 * kk][1]);
+        a[kk][1] = pack_bf16x2(c[2 * kk][2], c[2 * kk][3]);
+        a[kk][2] = pack_bf16x2(c[2 * kk + 1][0], c[2 * kk + 1][1]);
+        a[kk][3] = pack_bf16x2(c[2 * kk + 1][2], c[2 * kk + 1][3]);
+    }
+}
+
+template <int HDP>
+__global__ void __launch_bounds__(256, 1) attn_bwd_dq_kernel(const AttnBwdParams p) {
+    using C = BwdDqSmem<HDP>;
+    constexpr int NT = HDP / 8;
+    extern __shared__ __align__(128) uint8_t smem[];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int g = lane >> 2, t = lane & 3;
+    const int q0 = blockIdx.x * 128, h = blockIdx.y, b = blockIdx.z;
+    const uint32_t sQ = smem_u32(smem), sDo = sQ + C::kDoOff, sK = sQ + C::kKOff, sV = sQ + C::kVOff;
+    const int nb0 = (p.kv[0].len + 63) / 64;
+    const int nb1 = p.kv[1].len > 0 ? (p.kv[1].len + 63) / 64 : 0;
     const int T = nb0 + nb1;
 
-    if (threadIdx.x == 0) {
-        tma_prefetch_desc(&tmQ);
-        tma_prefetch_desc(&tmDO);
-        tma_prefetch_desc(&tmK0);
-        tma_prefetch_desc(&tmV0);
-        mbar_init(q_full, 1);
-        for (int i = 0; i < KV_STAGES; ++i) {
-            mbar_init(&kv_full[i], 1);
-            mbar_init(&kv_empty[i], 1);
-        }
-        mbar_init(s_full, 1);
-        mbar_init(o_full, 1);
-        mbar_init(s_free, 256);
-        for (int i = 0; i < DSB; ++i) {
-            mbar_init(&p_full[i], 256);
-            mbar_init(&pv_done[i], 1);
-        }
-        fence_barrier_init();
-    }
-    if (warp == 9) {
-        tmem_alloc(tmem_slot, 512);
-        tmem_relinquish();
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    const uint32_t tmem_S = tmem_base;
-    const uint32_t tmem_dP = tmem_base + 128;
-    const uint32_t tmem_dQ = tmem_base + 256;
+    attn_load_rows<HDP>(sQ, p.q + static_cast<int64_t>(b) * p.Lq * p.q_ld + h * p.hd, p.q_ld, p.hd, q0, p.Lq, 128);
+    attn_load_rows<HDP>(sDo, p.d_out + static_cast<int64_t>(b) * p.Lq * p.do_ld + h * p.hd, p.do_ld, p.hd, q0, p.Lq, 128);
+    auto load_kv = [&](int i) {
+        const int s = i < nb0 ? 0 : 1;
+        const int j = s ? i - nb0 : i;
+        const AttnKV& kv = p.kv[s];
+        const int64_t base = static_cast<int64_t>(b) * kv.sample_rows * kv.ld + h * p.hd;
+        attn_load_rows<HDP>(sK + (i & 1) * C::kKVBytes, kv.k + base, kv.ld, p.hd, j * 64, kv.len, 64);
+        attn_load_rows<HDP>(sV + (i & 1) * C::kKVBytes, kv.v + base, kv.ld, p.hd, j * 64, kv.len, 64);
+    };
+    load_kv(0);
+    cp_async_commit();
 
-    if (warp == 8) {
-        // ------------------------------------------------ TMA producer
-        if (elect_one()) {
-            mbar_arrive_expect_tx(q_full, 2 * NATOM * kBAtom);
+    const int row0 = q0 + warp * 16 + g;
+    float dq[NT][4];
 #pragma unroll
-            for (int a = 0; a < NATOM; ++a) {
-                tma_load_4d(sQ + a * kBAtom, &tmQ, q_full, a * 64, h, q0, b);
-                tma_load_4d(sDO + a * kBAtom, &tmDO, q_full, a * 64, h, q0, b);
-            }
-            for (int i = 0; i < T; ++i) {
-                const int s = i < nb0 ? 0 : 1;
-                const int j = s ? i - nb0 : i;
-                const int st = i % KV_STAGES;
-                const uint32_t ph = (i / KV_STAGES) & 1;
-                const CUtensorMap* mk = s ? &tmK1 : &tmK0;
-                const CUtensorMap* mv = s ? &tmV1 : &tmV0;
-                mbar_wait(&kv_empty[st], ph ^ 1);
-                mbar_arrive_expect_tx(&kv_full[st], 2 * NATOM * kBAtom);
+    for (int n = 0; n < NT; ++n) dq[n][0] = dq[n][1] = dq[n][2] = dq[n][3] = 0.f;
+    for (int i = 0; i < T; ++i) {
+        const int s = i < nb0 ? 0 : 1;
+        const int j = s ? i - nb0 : i;
+        const float w = s ? p.w1 : p.w0;
+        float lse[2], dd[2];
 #pragma unroll
-                for (int a = 0; a < NATOM; ++a) {
-                    tma_load_4d(sK + (st * NATOM + a) * kBAtom, mk, &kv_full[st], a * 64, h, j * 128, b);
-                    tma_load_4d(sV + (st * NATOM + a) * kBAtom, mv, &kv_full[st], a * 64, h, j * 128, b);
-                }
+        for (int hr = 0; hr < 2; ++hr) {
+            const int q = row0 + hr * 8;
+            const int64_t idx = ((static_cast<int64_t>(s) * p.B + b) * p.heads + h) * p.lq_pad + q;
+            lse[hr] = q < p.Lq ? __ldg(p.lse + idx) : INFINITY;
+            dd[hr] = q < p.Lq ? __ldg(p.dsum + idx) : 0.f;
+        }
+        cp_async_wait<0>();
+        __syncthreads();
+        if (i + 1 < T) load_kv(i + 1);
+        cp_async_commit();
+        const uint32_t kb = sK + (i & 1) * C::kKVBytes, vb = sV + (i & 1) * C::kKVBytes;
+        float sc[8][4], dp[8][4];
+        bwd_mma_abt<HDP>(sc, sQ, warp * 16, kb, lane);
+        bwd_mma_abt<HDP>(dp, sDo, warp * 16, vb, lane);
+        const int len = p.kv[s].len;
+#pragma unroll
+        for (int n = 0; n < 8; ++n) {
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const int key = j * 64 + n * 8 + 2 * t + (e & 1);
+                const float pr = key < len ? ex2_approx(sc[n][e] * p.scale_log2 - lse[e >> 1]) : 0.f;
+                sc[n][e] = pr * (w * dp[n][e] - dd[e >> 1]);
             }
         }
-    } else if (warp == 9) {
-        // ------------------------------------------------ MMA issuer
-        if (elect_one()) {
-            constexpr uint32_t idesc_s = umma_idesc_bf16(128, 128, 0, 0);     // Q / dO (K-major) x K / V (K-major)
-            constexpr uint32_t idesc_o = umma_idesc_bf16(128, HD_MMA, 0, 1);  // dS (K-major) x K (MN-major)
-            constexpr bool kEarly = KV_STAGES > 1;
-            auto issue_s = [&](int i) {
-                const int st = i % KV_STAGES;
-                mbar_wait(&kv_full[st], (i / KV_STAGES) & 1);
-                tc_fence_after();
-                const uint32_t q_addr = smem_u32(sQ), do_addr = smem_u32(sDO);
-                const uint32_t k_addr = smem_u32(sK + st * NATOM * kBAtom), v_addr = smem_u32(sV + st * NATOM * kBAtom);
-#pragma unroll
-                for (int ks = 0; ks < HD_MMA / 16; ++ks) {
-                    const uint32_t off = (ks / 4) * kBAtom + (ks % 4) * 32;
-                    umma_bf16(tmem_S, umma_smem_desc_sw128(q_addr + off, 16, 1024),
-                              umma_smem_desc_sw128(k_addr + off, 16, 1024), idesc_s, ks > 0 ? 1u : 0u);
-                }
-#pragma unroll
-                for (int ks = 0; ks < HD_MMA / 16; ++ks) {
-                    const uint32_t off = (ks / 4) * kBAtom + (ks % 4) * 32;
-                    umma_bf16(tmem_dP, umma_smem_desc_sw128(do_addr + off, 16, 1024),
-                              umma_smem_desc_sw128(v_addr + off, 16, 1024), idesc_s, ks > 0 ? 1u : 0u);
-                }
-                umma_commit(s_full);
-            };
-            mbar_wait(q_full, 0);
-            issue_s(0);
-            for (int i = 0; i < T; ++i) {
-                const int st = i % KV_STAGES;
-                if (kEarly && i + 1 < T) {
-                    mbar_wait(s_free, i & 1);
-                    tc_fence_after();
-                    issue_s(i + 1);
-                }
-                // block i uses dS buffer i % DSB: its barriers see every DSB-th block, phase index i / DSB
-                mbar_wait(&p_full[i % DSB], (i / DSB) & 1);
-                tc_fence_after();
-                const uint32_t ds_addr = smem_u32(sDS) + (i % DSB) * 2 * kBAtom;
-                const uint32_t k_addr = smem_u32(sK + st * NATOM * kBAtom);
-#pragma unroll
-                for (int ks = 0; ks < 8; ++ks) {
-                    const uint32_t poff = (ks / 4) * kBAtom + (ks % 4) * 32;
-                    umma_bf16(tmem_dQ, umma_smem_desc_sw128(ds_addr + poff, 16, 1024),
-                              umma_smem_desc_sw128(k_addr + ks * 2048, kBAtom, 1024), idesc_o, (i > 0 || ks > 0) ? 1u : 0u);
-                }
-                umma_commit(&kv_empty[st]);
-                umma_commit(&pv_done[i % DSB]);
-                if (!kEarly && i + 1 < T) {
-                    mbar_wait(s_free, i & 1);
-                    tc_fence_after();
-                    issue_s(i + 1);
-                }
-            }
-            umma_commit(o_full);
-        }
-        __syncwarp();
-    } else {
-        // ------------------------------------------------ dS warps (0-7): TMEM lane = query row; halves split the 128 keys
-        const int lane = threadIdx.x & 31;
-        const int lg = warp & 3;
-        const int half = warp >> 2;
-        const int r = lg * 32 + lane;
-        const uint32_t lane_addr = static_cast<uint32_t>(lg * 32) << 16;
-        const uint32_t ds_row0 = smem_u32(sDS) + half * kBAtom + (r >> 3) * 1024 + (r & 7) * 128;
-        const uint32_t rx = r & 7;
-        const int q = q0 + r;
-        const int64_t vec = (static_cast<int64_t>(b) * p.heads + h) * p.lq_pad + min(q, p.lq_pad - 1);
-        const int64_t per = static_cast<int64_t>(p.B) * p.heads * p.lq_pad;
-        float lse = 0.f, dsum = 0.f, w = 0.f;
-        for (int i = 0; i < T; ++i) {
-            const int s = i < nb0 ? 0 : 1;
-            const int j = s ? i - nb0 : i;
-            if (j == 0) {
-                lse = q < p.Lq ? __ldg(p.lse + s * per + vec) : INFINITY;
-                dsum = q < p.Lq ? __ldg(p.dsum + s * per + vec) : 0.f;
-                w = s ? p.w1 : p.w0;
-            }
-            const int valid = (s ? p.len1 : p.len0) - j * 128 - half * 64;  // valid key columns in my half (may be <= 0)
-            bwd_wait(s_full, i & 1, p.spin);
-            tc_fence_after();
-#pragma unroll
-            for (int cc = 0; cc < 2; ++cc) {
-                uint32_t va[32], vb[32];
-                tmem_ld32(tmem_S + lane_addr + half * 64 + cc * 32, va);
-                tmem_ld32(tmem_dP + lane_addr + half * 64 + cc * 32, vb);
-                tmem_ld_wait();
-                if (cc == 1) {  // S / dP of this block are in registers: the tensor core may overwrite them
-                    tc_fence_before();
-                    mbar_arrive(s_free);
-                }
-                if (cc == 0 && i >= DSB) {  // the dQ += dS K that read this dS buffer (block i - DSB) must have retired
-                    bwd_wait(&pv_done[i % DSB], ((i / DSB) - 1) & 1, p.spin);
-                    tc_fence_after();
-                }
-#pragma unroll
-                for (int g = 0; g < 4; ++g) {
-                    float e[8];
-#pragma unroll
-                    for (int k = 0; k < 8; ++k) {
-                        const int col = cc * 32 + g * 8 + k;
-                        const float pr = ex2_approx(fmaf(__uint_as_float(va[g * 8 + k]), p.scale_log2, -lse));
-                        const float ds = pr * fmaf(w, __uint_as_float(vb[g * 8 + k]), -dsum);
-                        e[k] = col < valid ? ds : 0.f;
-                    }
-                    const uint32_t chunk = static_cast<uint32_t>(cc * 4 + g) ^ rx;
-                    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(ds_row0 + (i % DSB) * 2 * kBAtom + chunk * 16),
-                                 "r"(bwd_pack<PACK>(e[0], e[1])), "r"(bwd_pack<PACK>(e[2], e[3])),
-                                 "r"(bwd_pack<PACK>(e[4], e[5])), "r"(bwd_pack<PACK>(e[6], e[7]))
-                                 : "memory");
-                }
-            }
-            fence_proxy_async_smem();
-            tc_fence_before();
-            mbar_arrive(&p_full[i % DSB]);
-        }
-        // ---- epilogue: dQ = sm_scale * acc
-        mbar_wait(o_full, 0);
-        tc_fence_after();
-        constexpr int kChunks = HD_MMA / 16;
-        const int ch_begin = half == 0 ? 0 : (kChunks + 1) / 2;
-        const int ch_end = half == 0 ? (kChunks + 1) / 2 : kChunks;
-        __nv_bfloat16* orow =
-            reinterpret_cast<__nv_bfloat16*>(p.dq) + (static_cast<int64_t>(b) * p.Lq + q) * p.dq_ld + h * p.hd;
-#pragma unroll 1
-        for (int cc = ch_begin; cc < ch_end; ++cc) {
-            const int c = cc * 16;
-            uint32_t o[16];
-            tmem_ld16(tmem_dQ + lane_addr + c, o);
-            tmem_ld_wait();
-            if (q < p.Lq && c < p.hd) {
-                float f[16];
-#pragma unroll
-                for (int k = 0; k < 16; ++k) f[k] = p.sm_scale * __uint_as_float(o[k]);
-                uint4* dst = reinterpret_cast<uint4*>(orow + c);
-                dst[0] = make_uint4(pack_bf16x2(f[0], f[1]), pack_bf16x2(f[2], f[3]), pack_bf16x2(f[4], f[5]),
-                                    pack_bf16x2(f[6], f[7]));
-                if (c + 8 < p.hd)
-                    dst[1] = make_uint4(pack_bf16x2(f[8], f[9]), pack_bf16x2(f[10], f[11]), pack_bf16x2(f[12], f[13]),
-                                        pack_bf16x2(f[14], f[15]));
-            }
-        }
+        uint32_t a[4][4];
+        bwd_pack_a(sc, a);
+        bwd_mma_ab<HDP>(dq, a, kb, lane);
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 9) tmem_dealloc(tmem_base, 512);
+    attn_store_frag<NT>(dq, p.sm_scale, p.sm_scale, reinterpret_cast<__nv_bfloat16*>(p.dq), p.dq_ld,
+                        static_cast<int64_t>(b) * p.Lq, p.Lq, h, p.hd, row0, t);
 }
 
 // ------------------------------------------------------------------------------------------------ dK / dV kernel
-template <int HD_MMA, int NATOM, int QB, int STAGES, int CTAS = 1, int DSB = 1>
-struct DkvCfg {
-    static constexpr int kQAtom = QB * 128;  // one [QB rows x 64 bf16] swizzled tile of Q / dO
-    static constexpr int kPAtoms = QB / 64;  // P^T / dS^T: [128 keys x QB] = QB / 64 atoms of [128 x 64]
-    static constexpr int kKOff = 0;
-    static constexpr int kVOff = NATOM * kBAtom;
-    static constexpr int kQOff = 2 * NATOM * kBAtom;
-    static constexpr int kDoOff = kQOff + STAGES * NATOM * kQAtom;
-    static constexpr int kPOff = kDoOff + STAGES * NATOM * kQAtom;
-    static constexpr int kDsOff = kPOff + DSB * kPAtoms * kBAtom;  // DSB buffers each of P^T and dS^T
-    static constexpr int kVecOff = kDsOff + DSB * kPAtoms * kBAtom;  // per stage: lse2[QB] | D[QB] fp32
-    static constexpr int kBarOff = kVecOff + STAGES * 2 * QB * 4;
-    static constexpr int kNumBars = 1 + 2 * STAGES + 3 + 2 * DSB;
-    static constexpr int kTotal = kBarOff + kNumBars * 8 + 16;
-    static constexpr int kAccStride = (HD_MMA + 63) / 64 * 64;
-    static constexpr int kTmemDv = 2 * QB;
-    static constexpr int kTmemDk = 2 * QB + kAccStride;
-    static constexpr int kTmemCols = CTAS == 2 ? 256 : 512;  // two co-resident CTAs share the SM's 512 columns
-    static_assert(kTotal * CTAS <= 232448 - (CTAS - 1) * 2048, "dkv kernel: shared memory");
-    static_assert(kTmemDk + HD_MMA <= kTmemCols, "dkv kernel: TMEM");
+// CTA = 128 keys of one (sample, head) of ONE stream, 8 warps of 16 keys; Q / dO blocks of 64 queries stream through a
+// two-stage ring. The products are taken transposed (row = key): S^T = K Q^T, dP^T = V dO^T, P^T = exp2(S^T s log2e -
+// lse2[q]), dS^T = P^T o (w dP^T - D[q]), then dV += P^T dO and dK += dS^T Q with P^T / dS^T as register A fragments.
+template <int HDP>
+struct BwdDkvSmem {
+    static constexpr int kKBytes = 128 * attn_row_bytes(HDP);
+    static constexpr int kQBytes = 64 * attn_row_bytes(HDP);
+    static constexpr int kVOff = kKBytes;
+    static constexpr int kQOff = 2 * kKBytes;
+    static constexpr int kDoOff = kQOff + 2 * kQBytes;
+    static constexpr int kVecOff = kDoOff + 2 * kQBytes;  // [2 stages][lse2 | D][64] fp32
+    static constexpr int kTotal = kVecOff + 2 * 2 * 64 * 4;
 };
 
-// CTAS = 2 (with QB = 64: 256 TMEM columns, ~100 KB of shared memory): two CTAs per SM, so one CTA's exponential phase runs
-// under the other's tensor-core / synchronisation phases — the forward kernel's two-CTAs-per-SM arrangement.
-// DSB = 2: P^T / dS^T double-buffered with their own barrier pairs, as in the dQ kernel.
-template <int HD_MMA, int NATOM, int QB, int STAGES, int CTAS = 1, int PACK = 0, int DSB = 1>
-__global__ void __launch_bounds__(320, CTAS)
-attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmDO,
-                    const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
-                    const AttnBwdParams p) {
-    using C = DkvCfg<HD_MMA, NATOM, QB, STAGES, CTAS, DSB>;
-    constexpr int kQA = C::kQAtom;
-    constexpr int kBufBytes = C::kPAtoms * kBAtom;  // one P^T (or dS^T) buffer
-    extern __shared__ __align__(1024) uint8_t smem[];
-    if (threadIdx.x == 0 && (smem_u32(smem) & 1023u) != 0) __trap();
-    uint8_t* sK = smem + C::kKOff;
-    uint8_t* sV = smem + C::kVOff;
-    uint8_t* sQ = smem + C::kQOff;
-    uint8_t* sDO = smem + C::kDoOff;
-    uint8_t* sP = smem + C::kPOff;
-    uint8_t* sDS = smem + C::kDsOff;
-    float* sVec = reinterpret_cast<float*>(smem + C::kVecOff);
-    uint64_t* kv_full = reinterpret_cast<uint64_t*>(smem + C::kBarOff);
-    uint64_t* q_full = kv_full + 1;
-    uint64_t* q_empty = q_full + STAGES;
-    uint64_t* s_full = q_empty + STAGES;
-    uint64_t* o_full = s_full + 1;
-    uint64_t* s_free = o_full + 1;
-    uint64_t* p_full = s_free + 1;       // [DSB]
-    uint64_t* pv_done = p_full + DSB;    // [DSB]
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(pv_done + DSB);
-
-    const int warp = threadIdx.x >> 5;
-    const int k0 = blockIdx.x * 128;
-    const int h = blockIdx.y;
-    const int b = blockIdx.z;
-    const int T = (p.Lq + QB - 1) / QB;
-    const int len = p.stream ? p.len1 : p.len0;
+template <int HDP>
+__global__ void __launch_bounds__(256, 1) attn_bwd_dkv_kernel(const AttnBwdParams p) {
+    using C = BwdDkvSmem<HDP>;
+    constexpr int NT = HDP / 8;
+    extern __shared__ __align__(128) uint8_t smem[];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int g = lane >> 2, t = lane & 3;
+    const int k0 = blockIdx.x * 128, h = blockIdx.y, b = blockIdx.z;
+    const uint32_t sK = smem_u32(smem), sV = sK + C::kVOff, sQ = sK + C::kQOff, sDo = sK + C::kDoOff;
+    float* s_vec = reinterpret_cast<float*>(smem + C::kVecOff);
+    const AttnKV& kv = p.kv[p.stream];
     const float w = p.stream ? p.w1 : p.w0;
+    const int T = (p.Lq + 63) / 64;
 
-    if (threadIdx.x == 0) {
-        tma_prefetch_desc(&tmQ);
-        tma_prefetch_desc(&tmDO);
-        tma_prefetch_desc(&tmK);
-        tma_prefetch_desc(&tmV);
-        mbar_init(kv_full, 1);
-        for (int i = 0; i < STAGES; ++i) {
-            mbar_init(&q_full[i], 1);
-            mbar_init(&q_empty[i], 1);
+    const int64_t kbase = static_cast<int64_t>(b) * kv.sample_rows * kv.ld + h * p.hd;
+    attn_load_rows<HDP>(sK, kv.k + kbase, kv.ld, p.hd, k0, kv.len, 128);
+    attn_load_rows<HDP>(sV, kv.v + kbase, kv.ld, p.hd, k0, kv.len, 128);
+    const int64_t vec_base = ((static_cast<int64_t>(p.stream) * p.B + b) * p.heads + h) * p.lq_pad;
+    auto load_q = [&](int i) {
+        attn_load_rows<HDP>(sQ + (i & 1) * C::kQBytes, p.q + static_cast<int64_t>(b) * p.Lq * p.q_ld + h * p.hd, p.q_ld,
+                            p.hd, i * 64, p.Lq, 64);
+        attn_load_rows<HDP>(sDo + (i & 1) * C::kQBytes, p.d_out + static_cast<int64_t>(b) * p.Lq * p.do_ld + h * p.hd,
+                            p.do_ld, p.hd, i * 64, p.Lq, 64);
+        if (threadIdx.x < 128) {
+            const int qq = i * 64 + (threadIdx.x & 63);
+            const bool ok = qq < p.Lq;
+            float* dst = s_vec + (i & 1) * 128 + threadIdx.x;
+            if (threadIdx.x < 64) *dst = ok ? __ldg(p.lse + vec_base + qq) : INFINITY;
+            else *dst = ok ? __ldg(p.dsum + vec_base + qq) : 0.f;
         }
-        mbar_init(s_full, 1);
-        mbar_init(o_full, 1);
-        mbar_init(s_free, 256);
-        for (int i = 0; i < DSB; ++i) {
-            mbar_init(&p_full[i], 256);
-            mbar_init(&pv_done[i], 1);
-        }
-        fence_barrier_init();
-    }
-    if (warp == 9) {
-        tmem_alloc(tmem_slot, C::kTmemCols);
-        tmem_relinquish();
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    const uint32_t tmem_S = tmem_base;
-    const uint32_t tmem_dP = tmem_base + QB;
-    const uint32_t tmem_dV = tmem_base + C::kTmemDv;
-    const uint32_t tmem_dK = tmem_base + C::kTmemDk;
-    const int64_t vec_base = (static_cast<int64_t>(p.stream) * p.B * p.heads + static_cast<int64_t>(b) * p.heads + h) * p.lq_pad;
+    };
+    load_q(0);
+    cp_async_commit();
 
-    if (warp == 8) {
-        // ------------------------------------------------ TMA producer
-        if (elect_one()) {
-            mbar_arrive_expect_tx(kv_full, 2 * NATOM * kBAtom);
+    float dk[NT][4], dv[NT][4];
 #pragma unroll
-            for (int a = 0; a < NATOM; ++a) {
-                tma_load_4d(sK + a * kBAtom, &tmK, kv_full, a * 64, h, k0, b);
-                tma_load_4d(sV + a * kBAtom, &tmV, kv_full, a * 64, h, k0, b);
-            }
-            for (int i = 0; i < T; ++i) {
-                const int st = i % STAGES;
-                const uint32_t ph = (i / STAGES) & 1;
-                mbar_wait(&q_empty[st], ph ^ 1);
-                mbar_arrive_expect_tx(&q_full[st], 2 * NATOM * kQA + 2 * QB * 4);
-#pragma unroll
-                for (int a = 0; a < NATOM; ++a) {
-                    tma_load_4d(sQ + (st * NATOM + a) * kQA, &tmQ, &q_full[st], a * 64, h, i * QB, b);
-                    tma_load_4d(sDO + (st * NATOM + a) * kQA, &tmDO, &q_full[st], a * 64, h, i * QB, b);
-                }
-                // lq_pad is a multiple of 128 >= Lq: the vector reads never leave the buffers
-                bulk_load_g2s(smem_u32(sVec + st * 2 * QB), p.lse + vec_base + i * QB, QB * 4, &q_full[st]);
-                bulk_load_g2s(smem_u32(sVec + st * 2 * QB + QB), p.dsum + vec_base + i * QB, QB * 4, &q_full[st]);
-            }
-        }
-    } else if (warp == 9) {
-        // ------------------------------------------------ MMA issuer
-        if (elect_one()) {
-            constexpr uint32_t idesc_s = umma_idesc_bf16(128, QB, 0, 0);      // K / V (K-major) x Q / dO (K-major)
-            constexpr uint32_t idesc_o = umma_idesc_bf16(128, HD_MMA, 0, 1);  // P^T / dS^T (K-major) x dO / Q (MN-major)
-            constexpr bool kEarly = STAGES > 1;
-            auto issue_s = [&](int i) {
-                const int st = i % STAGES;
-                mbar_wait(&q_full[st], (i / STAGES) & 1);
-                tc_fence_after();
-                const uint32_t k_addr = smem_u32(sK), v_addr = smem_u32(sV);
-                const uint32_t q_addr = smem_u32(sQ + st * NATOM * kQA), do_addr = smem_u32(sDO + st * NATOM * kQA);
-#pragma unroll
-                for (int ks = 0; ks < HD_MMA / 16; ++ks) {
-                    const uint32_t offa = (ks / 4) * kBAtom + (ks % 4) * 32;
-                    const uint32_t offb = (ks / 4) * kQA + (ks % 4) * 32;
-                    umma_bf16(tmem_S, umma_smem_desc_sw128(k_addr + offa, 16, 1024),
-                              umma_smem_desc_sw128(q_addr + offb, 16, 1024), idesc_s, ks > 0 ? 1u : 0u);
-                }
-#pragma unroll
-                for (int ks = 0; ks < HD_MMA / 16; ++ks) {
-                    const uint32_t offa = (ks / 4) * kBAtom + (ks % 4) * 32;
-                    const uint32_t offb = (ks / 4) * kQA + (ks % 4) * 32;
-                    umma_bf16(tmem_dP, umma_smem_desc_sw128(v_addr + offa, 16, 1024),
-                              umma_smem_desc_sw128(do_addr + offb, 16, 1024), idesc_s, ks > 0 ? 1u : 0u);
-                }
-                umma_commit(s_full);
-            };
-            mbar_wait(kv_full, 0);
-            issue_s(0);
-            for (int i = 0; i < T; ++i) {
-                const int st = i % STAGES;
-                if (kEarly && i + 1 < T) {
-                    mbar_wait(s_free, i & 1);
-                    tc_fence_after();
-                    issue_s(i + 1);
-                }
-                mbar_wait(&p_full[i % DSB], (i / DSB) & 1);
-                tc_fence_after();
-                const uint32_t p_addr = smem_u32(sP) + (i % DSB) * kBufBytes, ds_addr = smem_u32(sDS) + (i % DSB) * kBufBytes;
-                const uint32_t q_addr = smem_u32(sQ + st * NATOM * kQA), do_addr = smem_u32(sDO + st * NATOM * kQA);
-#pragma unroll
-                for (int ks = 0; ks < QB / 16; ++ks) {
-                    const uint32_t poff = (ks / 4) * kBAtom + (ks % 4) * 32;
-                    umma_bf16(tmem_dV, umma_smem_desc_sw128(p_addr + poff, 16, 1024),
-                              umma_smem_desc_sw128(do_addr + ks * 2048, kQA, 1024), idesc_o, (i > 0 || ks > 0) ? 1u : 0u);
-                }
-#pragma unroll
-                for (int ks = 0; ks < QB / 16; ++ks) {
-                    const uint32_t poff = (ks / 4) * kBAtom + (ks % 4) * 32;
-                    umma_bf16(tmem_dK, umma_smem_desc_sw128(ds_addr + poff, 16, 1024),
-                              umma_smem_desc_sw128(q_addr + ks * 2048, kQA, 1024), idesc_o, (i > 0 || ks > 0) ? 1u : 0u);
-                }
-                umma_commit(&q_empty[st]);
-                umma_commit(&pv_done[i % DSB]);
-                if (!kEarly && i + 1 < T) {
-                    mbar_wait(s_free, i & 1);
-                    tc_fence_after();
-                    issue_s(i + 1);
-                }
-            }
-            umma_commit(o_full);
-        }
-        __syncwarp();
-    } else {
-        // ------------------------------------------------ P^T / dS^T warps (0-7): TMEM lane = key row; halves split the QB queries
-        constexpr int kCols = QB / 2;      // query columns per thread
-        constexpr int kCC = kCols / 32;    // 32-column register chunks
-        const int lane = threadIdx.x & 31;
-        const int lg = warp & 3;
-        const int half = warp >> 2;
-        const int r = lg * 32 + lane;
-        const uint32_t lane_addr = static_cast<uint32_t>(lg * 32) << 16;
-        // my first column = half * kCols: atom (half * kCols) / 64, 16-byte chunk ((half * kCols) % 64) / 8 within the row
-        const uint32_t row_off = (r >> 3) * 1024 + (r & 7) * 128;
-        const uint32_t atom0 = (half * kCols) / 64, chunk0 = ((half * kCols) % 64) / 8;
-        const uint32_t p_row = smem_u32(sP) + atom0 * kBAtom + row_off;
-        const uint32_t ds_row = smem_u32(sDS) + atom0 * kBAtom + row_off;
-        const uint32_t rx = r & 7;
-        const bool key_ok = k0 + r < len;
-        for (int i = 0; i < T; ++i) {
-            const int st = i % STAGES;
-            const float* vl = sVec + st * 2 * QB + half * kCols;  // lse2 of my columns; D follows at + QB
-            // the lse2 / D vectors arrive by bulk copy on q_full[st]: observe that barrier directly (the MMA thread's wait
-            // does not order the async-proxy writes for this thread). The phase cannot advance twice under us: the slot is
-            // re-armed only after q_empty[st], which follows the p_full arrival of every thread here.
-            bwd_wait(&q_full[st], (i / STAGES) & 1, p.spin);
-            bwd_wait(s_full, i & 1, p.spin);
-            tc_fence_after();
-#pragma unroll
-            for (int cc = 0; cc < kCC; ++cc) {
-                uint32_t va[32], vb[32];
-                tmem_ld32(tmem_S + lane_addr + half * kCols + cc * 32, va);
-                tmem_ld32(tmem_dP + lane_addr + half * kCols + cc * 32, vb);
-                tmem_ld_wait();
-                if (cc == kCC - 1) {
-                    tc_fence_before();
-                    mbar_arrive(s_free);
-                }
-                if (cc == 0 && i >= DSB) {
-                    bwd_wait(&pv_done[i % DSB], ((i / DSB) - 1) & 1, p.spin);
-                    tc_fence_after();
-                }
-#pragma unroll
-                for (int g = 0; g < 4; ++g) {
-                    const float4 l0 = *reinterpret_cast<const float4*>(vl + cc * 32 + g * 8);
-                    const float4 l1 = *reinterpret_cast<const float4*>(vl + cc * 32 + g * 8 + 4);
-                    const float4 d0 = *reinterpret_cast<const float4*>(vl + QB + cc * 32 + g * 8);
-                    const float4 d1 = *reinterpret_cast<const float4*>(vl + QB + cc * 32 + g * 8 + 4);
-                    const float ls[8] = {l0.x, l0.y, l0.z, l0.w, l1.x, l1.y, l1.z, l1.w};
-                    const float dd[8] = {d0.x, d0.y, d0.z, d0.w, d1.x, d1.y, d1.z, d1.w};
-                    float pe[8], de[8];
-#pragma unroll
-                    for (int k = 0; k < 8; ++k) {
-                        float pr = ex2_approx(fmaf(__uint_as_float(va[g * 8 + k]), p.scale_log2, -ls[k]));
-                        pr = key_ok ? pr : 0.f;
-                        pe[k] = pr;
-                        de[k] = pr * fmaf(w, __uint_as_float(vb[g * 8 + k]), -dd[k]);
-                    }
-                    const uint32_t chunk = (chunk0 + static_cast<uint32_t>(cc * 4 + g)) ^ rx;
-                    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(p_row + (i % DSB) * kBufBytes + chunk * 16),
-                                 "r"(bwd_pack<PACK>(pe[0], pe[1])), "r"(bwd_pack<PACK>(pe[2], pe[3])),
-                                 "r"(bwd_pack<PACK>(pe[4], pe[5])), "r"(bwd_pack<PACK>(pe[6], pe[7]))
-                                 : "memory");
-                    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(ds_row + (i % DSB) * kBufBytes + chunk * 16),
-                                 "r"(bwd_pack<PACK>(de[0], de[1])), "r"(bwd_pack<PACK>(de[2], de[3])),
-                                 "r"(bwd_pack<PACK>(de[4], de[5])), "r"(bwd_pack<PACK>(de[6], de[7]))
-                                 : "memory");
-                }
-            }
-            fence_proxy_async_smem();
-            tc_fence_before();
-            mbar_arrive(&p_full[i % DSB]);
-        }
-        // ---- epilogue: dV = w * acc_dV, dK = sm_scale * acc_dK
-        mbar_wait(o_full, 0);
-        tc_fence_after();
-        constexpr int kChunks = HD_MMA / 16;
-        const int ch_begin = half == 0 ? 0 : (kChunks + 1) / 2;
-        const int ch_end = half == 0 ? (kChunks + 1) / 2 : kChunks;
-        const int64_t row = (static_cast<int64_t>(b) * p.kv_sample_rows + k0 + r) * p.dkv_ld + h * p.hd;
-#pragma unroll 1
-        for (int cc = ch_begin; cc < ch_end; ++cc) {
-            const int c = cc * 16;
-            uint32_t ov[16], ok[16];
-            tmem_ld16(tmem_dV + lane_addr + c, ov);
-            tmem_ld16(tmem_dK + lane_addr + c, ok);
-            tmem_ld_wait();
-            if (key_ok && c < p.hd) {
-#pragma unroll
-                for (int t = 0; t < 2; ++t) {
-                    const uint32_t(&o)[16] = t ? ok : ov;
-                    const float sc = t ? p.sm_scale : w;
-                    uint4* dst = reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(t ? p.dk : p.dv) + row + c);
-                    dst[0] = make_uint4(pack_bf16x2(sc * __uint_as_float(o[0]), sc * __uint_as_float(o[1])),
-                                        pack_bf16x2(sc * __uint_as_float(o[2]), sc * __uint_as_float(o[3])),
-                                        pack_bf16x2(sc * __uint_as_float(o[4]), sc * __uint_as_float(o[5])),
-                                        pack_bf16x2(sc * __uint_as_float(o[6]), sc * __uint_as_float(o[7])));
-                    if (c + 8 < p.hd)
-                        dst[1] = make_uint4(pack_bf16x2(sc * __uint_as_float(o[8]), sc * __uint_as_float(o[9])),
-                                            pack_bf16x2(sc * __uint_as_float(o[10]), sc * __uint_as_float(o[11])),
-                                            pack_bf16x2(sc * __uint_as_float(o[12]), sc * __uint_as_float(o[13])),
-                                            pack_bf16x2(sc * __uint_as_float(o[14]), sc * __uint_as_float(o[15])));
-                }
-            }
-        }
+    for (int n = 0; n < NT; ++n) {
+        dk[n][0] = dk[n][1] = dk[n][2] = dk[n][3] = 0.f;
+        dv[n][0] = dv[n][1] = dv[n][2] = dv[n][3] = 0.f;
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 9) tmem_dealloc(tmem_base, C::kTmemCols);
+    for (int i = 0; i < T; ++i) {
+        cp_async_wait<0>();
+        __syncthreads();
+        if (i + 1 < T) load_q(i + 1);
+        cp_async_commit();
+        const uint32_t qb = sQ + (i & 1) * C::kQBytes, dob = sDo + (i & 1) * C::kQBytes;
+        const float* lse = s_vec + (i & 1) * 128;
+        const float* dd = lse + 64;
+        float sc[8][4], dp[8][4];
+        bwd_mma_abt<HDP>(sc, sK, warp * 16, qb, lane);
+        bwd_mma_abt<HDP>(dp, sV, warp * 16, dob, lane);
+        uint32_t a[4][4];
+#pragma unroll
+        for (int n = 0; n < 8; ++n) {
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const int qc = n * 8 + 2 * t + (e & 1);  // query column within the block
+                const float pr = ex2_approx(sc[n][e] * p.scale_log2 - lse[qc]);
+                sc[n][e] = pr;
+                dp[n][e] = pr * (w * dp[n][e] - dd[qc]);
+            }
+        }
+        bwd_pack_a(sc, a);
+        bwd_mma_ab<HDP>(dv, a, dob, lane);
+        bwd_pack_a(dp, a);
+        bwd_mma_ab<HDP>(dk, a, qb, lane);
+    }
+    const int key0 = k0 + warp * 16 + g;
+    const int64_t rb = static_cast<int64_t>(b) * p.kv_sample_rows;
+    attn_store_frag<NT>(dv, w, w, reinterpret_cast<__nv_bfloat16*>(p.dv), p.dkv_ld, rb, kv.len, h, p.hd, key0, t);
+    attn_store_frag<NT>(dk, p.sm_scale, p.sm_scale, reinterpret_cast<__nv_bfloat16*>(p.dk), p.dkv_ld, rb, kv.len, h, p.hd,
+                        key0, t);
 }
 
 // ------------------------------------------------------------------------------------------------ D = w * rowsum(dO o O_s)
@@ -645,35 +295,44 @@ __global__ void attn_bwd_prep_kernel(const __nv_bfloat16* __restrict__ d_out, in
 }
 
 // ------------------------------------------------------------------------------------------------ host side
-static int make_tmap_rows(CUtensorMap* tm, const void* base, int64_t ld, int hd, int heads, int len, int nsamples,
-                          int sample_rows, int box_rows) {
-    uint64_t dims[4] = {static_cast<uint64_t>(hd), static_cast<uint64_t>(heads), static_cast<uint64_t>(len),
-                        static_cast<uint64_t>(nsamples)};
-    uint64_t strides[3] = {static_cast<uint64_t>(hd) * 2, static_cast<uint64_t>(ld) * 2,
-                           static_cast<uint64_t>(ld) * 2 * (sample_rows > 0 ? sample_rows : len)};
-    uint32_t box[4] = {64, 1, static_cast<uint32_t>(box_rows), 1};
-    return make_tmap_bf16(tm, base, 4, dims, strides, box);
-}
-
-template <int HD_MMA, int NATOM, int KV_STAGES, int PACK = 0, int DSB = 1>
-static int launch_dq(const CUtensorMap* tms, const AttnBwdParams& p, cudaStream_t stream) {
-    using C = DqCfg<HD_MMA, NATOM, KV_STAGES, DSB>;
-    IMAGD_SET_MAX_SMEM((attn_bwd_dq_kernel<HD_MMA, NATOM, KV_STAGES, PACK, DSB>), C::kTotal);
+template <int HDP>
+static int launch_dq(const AttnBwdParams& p, cudaStream_t stream) {
+    using C = BwdDqSmem<HDP>;
+    IMAGD_SET_MAX_SMEM(attn_bwd_dq_kernel<HDP>, C::kTotal);
     dim3 grid((p.Lq + 127) / 128, p.heads, p.B);
-    attn_bwd_dq_kernel<HD_MMA, NATOM, KV_STAGES, PACK, DSB><<<grid, 320, C::kTotal, stream>>>(tms[0], tms[1], tms[2], tms[3],
-                                                                                              tms[4], tms[5], p);
+    attn_bwd_dq_kernel<HDP><<<grid, 256, C::kTotal, stream>>>(p);
     IMAGD_LAUNCH_CHECK("attn_bwd_dq_kernel");
     return IMAGD_OK;
 }
 
-template <int HD_MMA, int NATOM, int QB, int STAGES, int CTAS = 1, int PACK = 0, int DSB = 1>
-static int launch_dkv(const CUtensorMap& tq, const CUtensorMap& tdo, const CUtensorMap& tk, const CUtensorMap& tv,
-                      const AttnBwdParams& p, int len, cudaStream_t stream) {
-    using C = DkvCfg<HD_MMA, NATOM, QB, STAGES, CTAS, DSB>;
-    IMAGD_SET_MAX_SMEM((attn_bwd_dkv_kernel<HD_MMA, NATOM, QB, STAGES, CTAS, PACK, DSB>), C::kTotal);
+template <int HDP>
+static int launch_dkv(const AttnBwdParams& p, int len, cudaStream_t stream) {
+    using C = BwdDkvSmem<HDP>;
+    IMAGD_SET_MAX_SMEM(attn_bwd_dkv_kernel<HDP>, C::kTotal);
     dim3 grid((len + 127) / 128, p.heads, p.B);
-    attn_bwd_dkv_kernel<HD_MMA, NATOM, QB, STAGES, CTAS, PACK, DSB><<<grid, 320, C::kTotal, stream>>>(tq, tdo, tk, tv, p);
+    attn_bwd_dkv_kernel<HDP><<<grid, 256, C::kTotal, stream>>>(p);
     IMAGD_LAUNCH_CHECK("attn_bwd_dkv_kernel");
+    return IMAGD_OK;
+}
+
+template <int HDP>
+static int launch_bwd(AttnBwdParams p, void* dk0, void* dv0, int64_t dkv0_ld, void* dk1, void* dv1, int64_t dkv1_ld,
+                      cudaStream_t stream) {
+    if (p.dq != nullptr) {
+        const int rc = launch_dq<HDP>(p, stream);
+        if (rc != IMAGD_OK) return rc;
+    }
+    for (int s = 0; s < 2; ++s) {
+        void* dk = s ? dk1 : dk0;
+        if (dk == nullptr) continue;
+        p.stream = s;
+        p.dk = dk;
+        p.dv = s ? dv1 : dv0;
+        p.dkv_ld = s ? dkv1_ld : dkv0_ld;
+        p.kv_sample_rows = p.kv[s].sample_rows;
+        const int rc = launch_dkv<HDP>(p, p.kv[s].len, stream);
+        if (rc != IMAGD_OK) return rc;
+    }
     return IMAGD_OK;
 }
 
@@ -722,8 +381,21 @@ extern "C" int imagd_attention_bwd_bf16(const void* q, int64_t q_ld, const void*
     p.hd = head_dim;
     p.sm_scale = sm_scale;
     p.scale_log2 = sm_scale * 1.4426950408889634f;
-    p.len0 = s0->len;
-    p.len1 = has1 ? s1->len : 0;
+    p.q = static_cast<const __nv_bfloat16*>(q);
+    p.q_ld = q_ld;
+    p.d_out = static_cast<const __nv_bfloat16*>(d_out);
+    p.do_ld = do_ld;
+    IMAGD_CHECK_ARG(q_ld % 8 == 0 && do_ld % 8 == 0 && aligned16(q) && aligned16(d_out), "attention_bwd: Q / dO alignment");
+    for (int s = 0; s < 2; ++s) {
+        const imagd_kv_stream* ks = s ? s1 : s0;
+        if (s == 1 && !has1) break;
+        IMAGD_CHECK_ARG(ks->ld % 8 == 0 && aligned16(ks->k) && aligned16(ks->v), "attention_bwd: K / V alignment");
+        p.kv[s].k = static_cast<const __nv_bfloat16*>(ks->k);
+        p.kv[s].v = static_cast<const __nv_bfloat16*>(ks->v);
+        p.kv[s].ld = ks->ld;
+        p.kv[s].len = ks->len;
+        p.kv[s].sample_rows = ks->sample_rows > 0 ? ks->sample_rows : ks->len;
+    }
     p.w0 = s0->out_scale;
     p.w1 = has1 ? s1->out_scale : 0.f;
     p.lq_pad = lq_pad;
@@ -731,92 +403,11 @@ extern "C" int imagd_attention_bwd_bf16(const void* q, int64_t q_ld, const void*
     p.dsum = dsum;
     p.dq = dq;
     p.dq_ld = dq_ld;
-    static const int spin = [] { const char* e = getenv("IMAGD_BWD_SPIN"); return e ? atoi(e) : 0; }();
-    p.spin = spin;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-
-    if (dq != nullptr) {
-        CUtensorMap tms[6];
-        int rc = make_tmap_rows(&tms[0], q, q_ld, head_dim, heads, Lq, B, 0, 128);
-        if (rc != IMAGD_OK) return rc;
-        rc = make_tmap_rows(&tms[1], d_out, do_ld, head_dim, heads, Lq, B, 0, 128);
-        if (rc != IMAGD_OK) return rc;
-        rc = make_tmap_rows(&tms[2], s0->k, s0->ld, head_dim, heads, s0->len, B, s0->sample_rows, 128);
-        if (rc != IMAGD_OK) return rc;
-        rc = make_tmap_rows(&tms[3], s0->v, s0->ld, head_dim, heads, s0->len, B, s0->sample_rows, 128);
-        if (rc != IMAGD_OK) return rc;
-        if (has1) {
-            rc = make_tmap_rows(&tms[4], s1->k, s1->ld, head_dim, heads, s1->len, B, s1->sample_rows, 128);
-            if (rc != IMAGD_OK) return rc;
-            rc = make_tmap_rows(&tms[5], s1->v, s1->ld, head_dim, heads, s1->len, B, s1->sample_rows, 128);
-            if (rc != IMAGD_OK) return rc;
-        } else {
-            tms[4] = tms[2];
-            tms[5] = tms[3];
-        }
-        static const int bwd_pack_mode = [] { const char* e = getenv("IMAGD_BWD_PACK"); return e ? atoi(e) : 0; }();
-        // K/V ring depth of the one-CTA-per-SM dQ kernel (head_dim 40 / 64): with two stages only ONE key block is in flight
-        // ahead of the tensor core and the ~1 us L2 -> shared latency of every block is exposed (measured ~4000 clk per
-        // block against 1024 clk of exponentials); IMAGD_BWD_DQ_STAGES=2 restores the shallow ring for A/B.
-        static const int dq_stages = [] { const char* e = getenv("IMAGD_BWD_DQ_STAGES"); return e ? atoi(e) : 4; }();
-        static const int dq_dsb = [] { const char* e = getenv("IMAGD_BWD_DQ_DSB"); return e ? atoi(e) : 2; }();
-        switch (head_dim) {
-            case 40:  // IMAGD_BWD_DQ_DSB=1 keeps the single dS buffer (A/B)
-                if (dq_stages >= 4) rc = dq_dsb >= 2 ? launch_dq<48, 1, 4, 0, 2>(tms, p, st) : launch_dq<48, 1, 4>(tms, p, st);
-                else rc = bwd_pack_mode == 2 ? launch_dq<48, 1, 2, 2>(tms, p, st) : launch_dq<48, 1, 2>(tms, p, st);
-                break;
-            case 64:
-                if (dq_stages >= 4) rc = dq_dsb >= 2 ? launch_dq<64, 1, 4, 0, 2>(tms, p, st) : launch_dq<64, 1, 4>(tms, p, st);
-                else rc = launch_dq<64, 1, 2>(tms, p, st);
-                break;
-            case 80: rc = launch_dq<80, 2, 2>(tms, p, st); break;
-            default: rc = launch_dq<160, 3, 1>(tms, p, st); break;
-        }
-        if (rc != IMAGD_OK) return rc;
+    switch (head_dim) {
+        case 40: return launch_bwd<48>(p, dk0, dv0, dkv0_ld, dk1, dv1, dkv1_ld, st);
+        case 64: return launch_bwd<64>(p, dk0, dv0, dkv0_ld, dk1, dv1, dkv1_ld, st);
+        case 80: return launch_bwd<80>(p, dk0, dv0, dkv0_ld, dk1, dv1, dkv1_ld, st);
+        default: return launch_bwd<160>(p, dk0, dv0, dkv0_ld, dk1, dv1, dkv1_ld, st);
     }
-    for (int s = 0; s < 2; ++s) {
-        void* dk = s ? dk1 : dk0;
-        void* dv = s ? dv1 : dv0;
-        if (dk == nullptr) continue;
-        const imagd_kv_stream* ks = s ? s1 : s0;
-        // head_dim 40 A/B switches: IMAGD_BWD_DKV2=1 -> 64-query blocks, two CTAs per SM; IMAGD_BWD_PACK=2 -> permute packing
-        // measured (profiles/r02_call16_attention_bwd_ab.txt, level-0 two-stream call, micro-batch 4): dK/dV kernel 785 -> 712 us
-        // with two CTAs per SM (default); the packing mode makes no difference (785 / 795, 712 / 713)
-        static const int dkv2 = [] { const char* e = getenv("IMAGD_BWD_DKV2"); return e ? atoi(e) : 1; }();
-        static const int pack_mode = [] { const char* e = getenv("IMAGD_BWD_PACK"); return e ? atoi(e) : 0; }();
-        const int qb = (head_dim <= 64 && !(head_dim == 40 && dkv2 > 0)) ? 128 : 64;
-        CUtensorMap tq, tdo, tk, tv;
-        int rc = make_tmap_rows(&tq, q, q_ld, head_dim, heads, Lq, B, 0, qb);
-        if (rc != IMAGD_OK) return rc;
-        rc = make_tmap_rows(&tdo, d_out, do_ld, head_dim, heads, Lq, B, 0, qb);
-        if (rc != IMAGD_OK) return rc;
-        rc = make_tmap_rows(&tk, ks->k, ks->ld, head_dim, heads, ks->len, B, ks->sample_rows, 128);
-        if (rc != IMAGD_OK) return rc;
-        rc = make_tmap_rows(&tv, ks->v, ks->ld, head_dim, heads, ks->len, B, ks->sample_rows, 128);
-        if (rc != IMAGD_OK) return rc;
-        p.stream = s;
-        p.dk = dk;
-        p.dv = dv;
-        p.dkv_ld = s ? dkv1_ld : dkv0_ld;
-        p.kv_sample_rows = ks->sample_rows > 0 ? ks->sample_rows : ks->len;
-        switch (head_dim) {
-            case 40:
-                if (dkv2 == 3)  // one CTA per SM, 64-query blocks, six-stage Q / dO ring, double-buffered P^T / dS^T
-                    rc = launch_dkv<48, 1, 64, 6, 1, 0, 2>(tq, tdo, tk, tv, p, ks->len, st);
-                else if (dkv2 > 0)
-                    rc = pack_mode == 2 ? launch_dkv<48, 1, 64, 2, 2, 2>(tq, tdo, tk, tv, p, ks->len, st)
-                                        : launch_dkv<48, 1, 64, 2, 2, 0>(tq, tdo, tk, tv, p, ks->len, st);
-                else if (dkv2 == 0)
-                    rc = pack_mode == 2 ? launch_dkv<48, 1, 128, 2, 1, 2>(tq, tdo, tk, tv, p, ks->len, st)
-                                        : launch_dkv<48, 1, 128, 2>(tq, tdo, tk, tv, p, ks->len, st);
-                else  // IMAGD_BWD_DKV2=-1: one CTA per SM, 128-query blocks, three-stage Q / dO ring
-                    rc = launch_dkv<48, 1, 128, 3>(tq, tdo, tk, tv, p, ks->len, st);
-                break;
-            case 64: rc = launch_dkv<64, 1, 128, 2>(tq, tdo, tk, tv, p, ks->len, st); break;
-            case 80: rc = launch_dkv<80, 2, 64, 2>(tq, tdo, tk, tv, p, ks->len, st); break;
-            default: rc = launch_dkv<160, 3, 64, 2>(tq, tdo, tk, tv, p, ks->len, st); break;
-        }
-        if (rc != IMAGD_OK) return rc;
-    }
-    return IMAGD_OK;
 }

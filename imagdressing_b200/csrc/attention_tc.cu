@@ -1,4 +1,4 @@
-// Two-stream ("hybrid") FlashAttention-style kernel on tcgen05 for sm_100a.
+// Two-stream ("hybrid") FlashAttention-style kernel for sm_90a.
 //
 //   out = w0 * softmax(Q K0^T * s) V0  +  w1 * softmax(Q K1^T * s) V1
 //
@@ -9,51 +9,30 @@
 // the Perceiver resampler).
 //
 // Data layout: Q/K/V stay in the projection GEMM's natural token-major output [rows, ld] (heads side by side in
-// the channel dim). TMA views them as (d, head, token, sample) and loads a 64-wide box per head; for
-// head_dim 40 / 80 / 160 the box over-runs the d extent and the hardware zero-fills, so no padded copies exist
-// in HBM and the MMA K extent is the head dim rounded to 16 (48 / 80 / 160).
+// the channel dim). Tiles are copied to shared memory with cp.async in 16-byte pieces; the head-dim columns
+// beyond hd (40 -> 48) and the rows beyond a stream's length are zero-filled, so no padded copies exist in HBM.
 //
-// CTA = 128 queries of one (sample, head). 320 threads:
-//   warps 0-7  softmax: TMEM lane = query row; warps w and w+4 own the same 32 rows and split the 128 score
-//              columns in halves (twice the warps to hide the exp / convert latency — at head_dim 40 the softmax,
-//              not the tensor pipe, bounds the kernel). S is read once with tcgen05.ld and held in registers, the two
-//              half-row maxima meet through 512 bytes of smem, P is written to smem in the UMMA K-major
-//              128B-swizzle layout, O is rescaled in TMEM only when the running max moves
-//   warp 8     TMA producer (K/V ring)
-//   warp 9     TMEM allocator + tcgen05.mma issuer:  S = Q K^T  (128x128xhd),  O_s += P V (128xhdx128)
-// TMEM columns: S [0,128), O_0 [128, +O_STRIDE), O_1 after it. Two CTAs per SM at head_dim 40 / 64.
-//
-// PT = true (head_dim 40 / 64, the two-CTAs-per-SM configurations): the probabilities never touch shared memory. Each
-// softmax thread packs its 64 exponentials to bf16 pairs and writes them with tcgen05.st over the first 64 columns of
-// its own S row (P aliases S), and P.V is a tcgen05.mma with the A operand in tensor memory. The round-1 profile of the
-// smem-P kernel (profiles/r01_ncu_attention_l0_v25.txt + the raw report) showed why: 15.2 M shared-store wavefronts +
-// 13.4 M tensor-core shared reads per launch (~60 % of the L1 data pipe), half of them P, and the MUFU.EX2 instructions
-// stalling on the MIO queue behind the 16-byte P stores. With P in TMEM the hot loop has no shared-memory store and no
-// generic->async proxy fence. S(i+1) = Q K(i+1)^T then has to follow P.V(i) (it overwrites P); the tensor-pipe gap
-// that leaves is covered by the second CTA on the SM.
+// CTA = 128 queries of one (sample, head), 8 warps of 16 query rows each. Key blocks of 64 rows stream through a
+// two-stage K / V ring; S = Q K^T and O += P V run on the tensor cores (mma.sync m16n8k16, bf16 -> fp32) with the
+// probabilities kept in registers (the S accumulator fragment is the P operand fragment). Online softmax in the log2
+// domain; when the first stream is done its weighted output w0 O0 / l0 waits in shared memory (fp32) for the second.
 #include <cstdlib>
-#include <type_traits>
 
 #include "common.cuh"
 #include "ptx.cuh"
-
-#ifndef IMAGD_ATTN_POLY
-#define IMAGD_ATTN_POLY 0  // r2-prep experiment knob: make EXTRA=-DIMAGD_ATTN_POLY=2
-#endif
+#include "attention_common.cuh"
 
 namespace imagd {
 
 struct AttnParams {
     int B, Lq, heads, hd;
     float scale_log2;  // sm_scale * log2(e)
-    int len0, len1;        // keys per sample of stream 0 / 1
-    int nq1;               // stream 1 applies to samples [0, nq1)
-    int bcast0, bcast1;
+    const __nv_bfloat16* q;
+    int64_t q_ld;
+    AttnKV kv[2];      // stream 0 / 1
+    int nq1;           // stream 1 applies to samples [0, nq1)
     float oscale0, oscale1;
-    int causal;            // stream 0 only: query q sees keys 0..q
-    int pdl_late;          // 1: release the dependent kernel when the last MMA is issued instead of at kernel entry
-    int pp_sync;           // ping-pong kernels: 1 = the two softmax groups alternate on the MUFU pipe through named barriers
-    int spin;              // ping-pong kernel: 1 = the softmax warps spin on s_full instead of suspending (IMAGD_ATTN_SPIN, A/B)
+    int causal;        // stream 0 only: query q sees keys 0..q
     void* out;
     int64_t out_ld;
     // training-mode extras (imagd_attention_train_fwd_bf16; all null / 0 on the inference path): per-row log-sum-exp of
@@ -65,562 +44,204 @@ struct AttnParams {
     int lq_pad;
 };
 
-constexpr int kAtomBytes = 128 * 128;  // one [128 rows x 64 bf16] swizzled tile
-
-template <int HD_MMA, int NATOM, int KV_STAGES, bool PT>
-struct AttnCfg {
-    static constexpr int kOStride = (HD_MMA + 63) / 64 * 64;
-    static constexpr int kTmemNeed = 128 + 2 * kOStride;
-    static constexpr int kTmemCols = kTmemNeed <= 256 ? 256 : 512;
-    static constexpr int kQBytes = NATOM * kAtomBytes;
+template <int HDP>
+struct AttnSmem {
+    static constexpr int kQBytes = 128 * attn_row_bytes(HDP);
+    static constexpr int kKVBytes = 64 * attn_row_bytes(HDP);  // one K or V block
     static constexpr int kKOff = kQBytes;
-    static constexpr int kVOff = kKOff + KV_STAGES * NATOM * kAtomBytes;
-    static constexpr int kPOff = kVOff + KV_STAGES * NATOM * kAtomBytes;
-    static constexpr int kPBytes = PT ? 2048 : 2 * kAtomBytes;  // PT: only the epilogue's row-sum exchange lives here
-    static constexpr int kBarOff = kPOff + kPBytes;
-    static constexpr int kNumBars = 1 + 3 * KV_STAGES + 5;  // q, k/v/empty per stage, s_full, p_full, o_full, s_free, pv_done
-    static constexpr int kMxOff = kBarOff + kNumBars * 8 + 16;  // [2 halves][128 rows] bf16 partial row maxima
-    static constexpr int kTotal = kMxOff + 512;
+    static constexpr int kVOff = kKOff + 2 * kKVBytes;
+    static constexpr int kOutOff = kVOff + 2 * kKVBytes;       // fp32 w0 O0 / l0 of the first stream, [HDP / 2][256 threads]
+    static constexpr int kTotal = kOutOff + HDP / 2 * 256 * 4;
 };
 
-template <int HD_MMA, int NATOM, int KV_STAGES, bool PT>
-__global__ void __launch_bounds__(320, (AttnCfg<HD_MMA, NATOM, KV_STAGES, PT>::kTmemCols <= 256 &&
-                                        AttnCfg<HD_MMA, NATOM, KV_STAGES, PT>::kTotal <= 113 * 1024) ? 2 : 1)
-attention_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK0,
-                    const __grid_constant__ CUtensorMap tmV0, const __grid_constant__ CUtensorMap tmK1,
-                    const __grid_constant__ CUtensorMap tmV1, const AttnParams p) {
-    using C = AttnCfg<HD_MMA, NATOM, KV_STAGES, PT>;
-    static_assert(!PT || C::kTmemCols == 256, "P-in-TMEM is built for the two-CTAs-per-SM configurations");
-    // HD_MMA == 48 only serves head_dim 40: columns 40..47 of every V tile are TMA zero fill. Column 40 is set to 1.0
-    // in shared memory, so O[:, 40] accumulates sum(P) on the tensor core — with exactly the bf16 rounding and the
-    // rescaling the output columns see — and the softmax warps neither add up nor exchange row sums.
-    constexpr bool kOnes = (HD_MMA == 48);
-    extern __shared__ __align__(1024) uint8_t smem[];  // SWIZZLE_128B tiles need 1024-byte alignment
-    if (threadIdx.x == 0 && (smem_u32(smem) & 1023u) != 0) {
-        printf("imagd: dynamic shared memory base %u is not 1024-byte aligned\n", smem_u32(smem));
-        __trap();
-    }
-    uint8_t* sQ = smem;
-    uint8_t* sK = smem + C::kKOff;
-    uint8_t* sV = smem + C::kVOff;
-    uint8_t* sP = smem + C::kPOff;
-    uint64_t* q_full = reinterpret_cast<uint64_t*>(smem + C::kBarOff);
-    uint64_t* k_full = q_full + 1;
-    uint64_t* v_full = k_full + KV_STAGES;
-    uint64_t* kv_empty = v_full + KV_STAGES;
-    uint64_t* s_full = kv_empty + KV_STAGES;
-    uint64_t* p_full = s_full + 1;
-    uint64_t* o_full = p_full + 1;
-    uint64_t* s_free = o_full + 1;   // all 256 softmax threads hold S(i) in registers: the tensor core may overwrite S
-    uint64_t* pv_done = s_free + 1;  // P.V(i) retired: P may be overwritten, O may be rescaled
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(pv_done + 1);
-
-    if (!p.pdl_late) pdl_launch_dependents();
-    const int warp = threadIdx.x >> 5;
-    const int lane = threadIdx.x & 31;
+template <int HDP>
+__global__ void __launch_bounds__(256, 1) attention_fwd_kernel(const AttnParams p) {
+    using C = AttnSmem<HDP>;
+    constexpr int kRow = attn_row_bytes(HDP);
+    constexpr int NT = HDP / 8;  // n8 tiles of O
+    extern __shared__ __align__(128) uint8_t smem[];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int q0 = blockIdx.x * 128;
     const int h = blockIdx.y;
     const int b = blockIdx.z;
+    const uint32_t sQ = smem_u32(smem), sK = sQ + C::kKOff, sV = sQ + C::kVOff;
+    float* s_out = reinterpret_cast<float*>(smem + C::kOutOff);
 
-    const int nb0 = (p.len0 + 127) / 128;
-    const int nb1 = (b < p.nq1) ? (p.len1 + 127) / 128 : 0;
+    const int nb0 = (p.kv[0].len + 63) / 64;
+    const int nb1 = (b < p.nq1) ? (p.kv[1].len + 63) / 64 : 0;
     const int T = nb0 + nb1;
 
-    if (threadIdx.x == 0) {
-        tma_prefetch_desc(&tmQ);
-        tma_prefetch_desc(&tmK0);
-        tma_prefetch_desc(&tmV0);
-        mbar_init(q_full, 1);
-        for (int i = 0; i < KV_STAGES; ++i) {
-            mbar_init(&k_full[i], 1);
-            mbar_init(&v_full[i], 1);
-            mbar_init(&kv_empty[i], 1);
-        }
-        mbar_init(s_full, 1);
-        mbar_init(p_full, 256);
-        mbar_init(o_full, 1);
-        mbar_init(s_free, 256);
-        mbar_init(pv_done, 1);
-        fence_barrier_init();
-    }
-    if (warp == 9) {
-        tmem_alloc(tmem_slot, C::kTmemCols);
-        tmem_relinquish();
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    const uint32_t tmem_S = tmem_base;
-    const uint32_t tmem_O = tmem_base + 128;
+    pdl_launch_dependents();
     pdl_wait();
+    attn_load_rows<HDP>(sQ, p.q + (static_cast<int64_t>(b) * p.Lq) * p.q_ld + h * p.hd, p.q_ld, p.hd, q0, p.Lq, 128);
+    auto load_kv = [&](int i) {
+        const int s = i < nb0 ? 0 : 1;
+        const int j = s ? i - nb0 : i;
+        const AttnKV& kv = p.kv[s];
+        const int64_t base = static_cast<int64_t>(kv.bcast ? 0 : b) * kv.sample_rows * kv.ld + h * p.hd;
+        attn_load_rows<HDP>(sK + (i & 1) * C::kKVBytes, kv.k + base, kv.ld, p.hd, j * 64, kv.len, 64);
+        attn_load_rows<HDP>(sV + (i & 1) * C::kKVBytes, kv.v + base, kv.ld, p.hd, j * 64, kv.len, 64);
+    };
+    load_kv(0);
+    cp_async_commit();
 
-    if (warp == 8) {
-        // ------------------------------------------------ TMA producer
-        if (elect_one()) {
-            mbar_arrive_expect_tx(q_full, C::kQBytes);
+    const int g = lane >> 2, t = lane & 3;
+    const int row0 = q0 + warp * 16 + g;  // this thread's query rows: row0, row0 + 8
+    float o[NT][4];
 #pragma unroll
-            for (int a = 0; a < NATOM; ++a) tma_load_4d(sQ + a * kAtomBytes, &tmQ, q_full, a * 64, h, q0, b);
-            for (int i = 0; i < T; ++i) {
-                const int s = i < nb0 ? 0 : 1;
-                const int j = s ? i - nb0 : i;
-                const int st = i % KV_STAGES;
-                const uint32_t ph = (i / KV_STAGES) & 1;
-                const CUtensorMap* mk = s ? &tmK1 : &tmK0;
-                const CUtensorMap* mv = s ? &tmV1 : &tmV0;
-                const int bk = (s ? p.bcast1 : p.bcast0) ? 0 : b;
-                mbar_wait(&kv_empty[st], ph ^ 1);
-                mbar_arrive_expect_tx(&k_full[st], NATOM * kAtomBytes);
-#pragma unroll
-                for (int a = 0; a < NATOM; ++a)
-                    tma_load_4d(sK + (st * NATOM + a) * kAtomBytes, mk, &k_full[st], a * 64, h, j * 128, bk);
-                mbar_arrive_expect_tx(&v_full[st], NATOM * kAtomBytes);
-#pragma unroll
-                for (int a = 0; a < NATOM; ++a)
-                    tma_load_4d(sV + (st * NATOM + a) * kAtomBytes, mv, &v_full[st], a * 64, h, j * 128, bk);
-            }
-        }
-    } else if (warp == 9) {
-        // ------------------------------------------------ MMA issuer (the whole warp plants the ones column in V)
-        const bool leader = elect_one();
-        constexpr uint32_t idesc_s = umma_idesc_bf16(128, 128, 0, 0);     // Q (K-major) x K (K-major)
-        constexpr uint32_t idesc_o = umma_idesc_bf16(128, HD_MMA, 0, 1);  // P (K-major) x V (MN-major)
-        // S(i+1) = Q K(i+1)^T is issued as soon as the softmax warps hold S(i) in registers (s_free), so the tensor
-        // core computes it underneath softmax(i); P.V(i) follows when P(i) is written. With a one-stage K/V ring
-        // (head_dim 160) the next K tile only lands after P.V(i) frees the slot, so QK(i+1) keeps the old order there.
-        constexpr bool kEarly = KV_STAGES > 1 && !PT;  // PT: S(i+1) overwrites P(i), so it is issued behind P.V(i)
-        auto issue_qk = [&](int i) {
-            const int st = i % KV_STAGES;
-            mbar_wait(&k_full[st], (i / KV_STAGES) & 1);
-            tc_fence_after();
-            const uint32_t q_addr = smem_u32(sQ);
-            const uint32_t k_addr = smem_u32(sK + st * NATOM * kAtomBytes);
-#pragma unroll
-            for (int ks = 0; ks < HD_MMA / 16; ++ks) {
-                const uint32_t off = (ks / 4) * kAtomBytes + (ks % 4) * 32;
-                umma_bf16(tmem_S, umma_smem_desc_sw128(q_addr + off, 16, 1024),
-                          umma_smem_desc_sw128(k_addr + off, 16, 1024), idesc_s, ks > 0 ? 1u : 0u);
-            }
-            umma_commit(s_full);
-        };
-        if (leader) {
-            mbar_wait(q_full, 0);
-            issue_qk(0);
-        }
-        __syncwarp();
-        for (int i = 0; i < T; ++i) {
-            const int s = i < nb0 ? 0 : 1;
-            const int j = s ? i - nb0 : i;
-            const int st = i % KV_STAGES;
-            const uint32_t ph = (i / KV_STAGES) & 1;
-            if (leader && kEarly && i + 1 < T) {
-                mbar_wait(s_free, i & 1);
-                tc_fence_after();
-                issue_qk(i + 1);
-            }
-            if constexpr (kOnes) {
-                // V[:, 40] = 1.0 (bf16 0x3F80): column 40 = 16-byte chunk 5 (swizzled by row), element 0. Overlaps softmax.
-                mbar_wait(&v_full[st], ph);
-                const uint32_t v_tile = smem_u32(sV + st * NATOM * kAtomBytes);
-#pragma unroll
-                for (int rr = 0; rr < 4; ++rr) {
-                    const uint32_t row = lane + rr * 32;
-                    const uint32_t addr = v_tile + (row >> 3) * 1024 + (row & 7) * 128 + ((5u ^ (row & 7)) << 4);
-                    asm volatile("st.shared.u16 [%0], %1;" ::"r"(addr), "h"(static_cast<unsigned short>(0x3F80)) : "memory");
-                }
-                fence_proxy_async_smem();
-            }
-            __syncwarp();
-            if (leader) {
-                mbar_wait(p_full, i & 1);
-                if constexpr (!kOnes) mbar_wait(&v_full[st], ph);
-                tc_fence_after();
-                const uint32_t p_addr = smem_u32(sP);
-                const uint32_t v_addr = smem_u32(sV + st * NATOM * kAtomBytes);
-                const uint32_t o_addr = tmem_O + s * C::kOStride;
-#pragma unroll
-                for (int ks = 0; ks < 8; ++ks) {
-                    if constexpr (PT) {  // A = P[:, 16 ks .. 16 ks + 15] = 8 packed columns of the S region
-                        umma_bf16_ts(o_addr, tmem_S + ks * 8, umma_smem_desc_sw128(v_addr + ks * 2048, kAtomBytes, 1024),
-                                     idesc_o, (j > 0 || ks > 0) ? 1u : 0u);
-                    } else {
-                        const uint32_t poff = (ks / 4) * kAtomBytes + (ks % 4) * 32;
-                        umma_bf16(o_addr, umma_smem_desc_sw128(p_addr + poff, 16, 1024),
-                                  umma_smem_desc_sw128(v_addr + ks * 2048, kAtomBytes, 1024), idesc_o,
-                                  (j > 0 || ks > 0) ? 1u : 0u);
-                    }
-                }
-                umma_commit(&kv_empty[st]);
-                umma_commit(pv_done);
-                if (!kEarly && i + 1 < T) {
-                    if constexpr (!PT) mbar_wait(s_free, i & 1);  // (already complete: P(i) was written after S(i) was read)
-                    issue_qk(i + 1);  // PT: the tensor pipe runs it behind P.V(i), which is done with P by then
-                }
-            }
-            __syncwarp();
-        }
-        if (leader) {
-            umma_commit(o_full);
-            if (p.pdl_late) pdl_launch_dependents();
-        }
-    } else {
-        // ------------------------------------------------ softmax / correction / epilogue (warps 0-7)
-        const int lg = warp & 3;          // TMEM lane quadrant
-        const int half = warp >> 2;       // which 64 score columns of the row this thread owns
-        const int r = lg * 32 + lane;     // query row in tile == TMEM lane
-        const uint32_t lane_addr = static_cast<uint32_t>(lg * 32) << 16;
-        __nv_bfloat16* mxbuf = reinterpret_cast<__nv_bfloat16*>(smem + C::kMxOff);
-        float m_run = -INFINITY, l_run = 0.f, l_first = 0.f, m_first = 0.f;
-        const uint32_t p_row = smem_u32(sP) + half * kAtomBytes + (r >> 3) * 1024 + (r & 7) * 128;
-        const uint32_t rx = r & 7;
-        // this thread's share of the O columns (16-column chunks) for the in-TMEM rescale and the epilogue
-        constexpr int kChunks = HD_MMA / 16;
-        const int ch_begin = half == 0 ? 0 : (kChunks + 1) / 2;
-        const int ch_end = half == 0 ? (kChunks + 1) / 2 : kChunks;
+    for (int n = 0; n < NT; ++n) o[n][0] = o[n][1] = o[n][2] = o[n][3] = 0.f;
+    float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+    float m_first[2] = {0.f, 0.f}, l_first[2] = {0.f, 0.f};
 
-        for (int i = 0; i < T; ++i) {
-            const int s = i < nb0 ? 0 : 1;
-            const int j = s ? i - nb0 : i;
-            if (j == 0 && i > 0) {
-                l_first = l_run;
-                m_first = m_run;
-                m_run = -INFINITY;
-                l_run = 0.f;
-            }
-            int valid = min(128, (s ? p.len1 : p.len0) - j * 128) - half * 64;  // valid columns in my half (may be <= 0)
-            if (p.causal) valid = min(valid, q0 + r + 1 - j * 128 - half * 64);   // keys 0..q of my row
-            // the full-tile fast path holds warp-collective TMEM stores: take it only when EVERY row of the warp is full
-            const bool full = __all_sync(0xffffffffu, valid >= 64);
-            mbar_wait(s_full, i & 1);
-            tc_fence_after();
-
-            // pass 1: my 64 scores -> registers (both 32-column loads in flight together), S is then released to the
-            // tensor core for the next key block; row maximum
-            float mx0 = -INFINITY, mx1 = -INFINITY, mx2 = -INFINITY, mx3 = -INFINITY;
-            uint32_t va[32], vb[32];
-            tmem_ld32(tmem_S + lane_addr + half * 64, va);
-            tmem_ld32(tmem_S + lane_addr + half * 64 + 32, vb);
-            tmem_ld_wait();
-            if constexpr (!PT) {
-                tc_fence_before();
-                mbar_arrive(s_free);  // my 64 scores live in registers from here on
-            }
-            if (full) {
+    for (int i = 0; i < T; ++i) {
+        const int s = i < nb0 ? 0 : 1;
+        const int j = s ? i - nb0 : i;
+        if (j == 0 && i > 0) {
+            // first stream done: park w0 * O0 / l0 (and the per-stream output of a training forward), restart for stream 1
 #pragma unroll
-                for (int k = 0; k < 32; k += 4) {
-                    mx0 = fmaxf(mx0, fmaxf(__uint_as_float(va[k]), __uint_as_float(vb[k])));
-                    mx1 = fmaxf(mx1, fmaxf(__uint_as_float(va[k + 1]), __uint_as_float(vb[k + 1])));
-                    mx2 = fmaxf(mx2, fmaxf(__uint_as_float(va[k + 2]), __uint_as_float(vb[k + 2])));
-                    mx3 = fmaxf(mx3, fmaxf(__uint_as_float(va[k + 3]), __uint_as_float(vb[k + 3])));
-                }
-            } else {
-#pragma unroll
-                for (int k = 0; k < 32; ++k) {
-                    if (k < valid) mx0 = fmaxf(mx0, __uint_as_float(va[k]));
-                    if (32 + k < valid) mx1 = fmaxf(mx1, __uint_as_float(vb[k]));
-                }
+            for (int hr = 0; hr < 2; ++hr) {
+                l_run[hr] = quad_sum(l_run[hr]);
+                m_first[hr] = m_run[hr];
+                l_first[hr] = l_run[hr];
             }
-            const float mx = fmaxf(fmaxf(mx0, mx1), fmaxf(mx2, mx3)) * p.scale_log2;
-            // Any m >= the true row max keeps exp2(s - m) <= 1, so the two half-row threads only have to agree on
-            // one: each publishes its maximum rounded UP to bf16 and both take the larger.
-            const __nv_bfloat16 mine = __float2bfloat16_ru(mx);
-            mxbuf[half * 128 + r] = mine;
-            // only the two warps that share these 32 rows have to meet (named barrier 1 + quadrant, 64 threads)
-            asm volatile("bar.sync %0, 64;" ::"r"(1 + lg) : "memory");
-            const float m_blk = fmaxf(__bfloat162float(mine), __bfloat162float(mxbuf[(half ^ 1) * 128 + r]));
-            // Lazy rescale: keep the old reference max unless the row max grew by more than 2^8. The probabilities are
-            // then bounded by 256 instead of 1 (exact in bf16 / fp32 all the same) and O / the row sum are rescaled
-            // only on the rare big jumps — the final O / l does not depend on which reference was used.
-            float m_new = fmaxf(m_run, m_blk);
-            if (m_new - m_run <= 8.0f) m_new = m_run;  // (-inf on a stream's first block: inf > 8 -> take m_blk)
-            const float alpha = ex2_approx(m_run - m_new);  // 0 on the first block of a stream
-            if (i > 0) {  // P.V(i-1) must have retired before P is overwritten or O rescaled (normally long done)
-                mbar_wait(pv_done, (i - 1) & 1);
-                tc_fence_after();
-            }
-            if (j > 0 && __any_sync(0xffffffffu, m_new > m_run)) {
-                // rescale my chunks of this stream's O accumulator in TMEM
-                const uint32_t o_addr = tmem_O + s * C::kOStride + lane_addr;
-#pragma unroll 1
-                for (int c = ch_begin; c < ch_end; ++c) {
-                    uint32_t o[16];
-                    tmem_ld16(o_addr + c * 16, o);
-                    tmem_ld_wait();
+            const float u0 = 1.f / l_run[0], u1 = 1.f / l_run[1];
 #pragma unroll
-                    for (int k = 0; k < 16; ++k) o[k] = __float_as_uint(__uint_as_float(o[k]) * alpha);
-                    tmem_st16(o_addr + c * 16, o);
-                }
-                tmem_st_wait();
+            for (int n = 0; n < NT; ++n) {
+                s_out[(n * 4 + 0) * 256 + threadIdx.x] = p.oscale0 * o[n][0] * u0;
+                s_out[(n * 4 + 1) * 256 + threadIdx.x] = p.oscale0 * o[n][1] * u0;
+                s_out[(n * 4 + 2) * 256 + threadIdx.x] = p.oscale0 * o[n][2] * u1;
+                s_out[(n * 4 + 3) * 256 + threadIdx.x] = p.oscale0 * o[n][3] * u1;
             }
-            m_run = m_new;
-
-            // pass 2: P = exp2(S*scale - m) for my 64 columns (still in registers) -> bf16 pairs; PT: written over the
-            // first 64 columns of my own S row in TMEM (32 packed columns per half), else one swizzled smem atom of P
-            float sum0 = 0.f, sum1 = 0.f, sum2 = 0.f, sum3 = 0.f;
-            const float sc = p.scale_log2;
-            // one branch per key block (full / ragged tile), not one per 8 columns
-            auto pass2 = [&](auto full_tag) {
-                constexpr bool kFull = decltype(full_tag)::value;
+            if (p.out_s0 != nullptr)
+                attn_store_frag<NT>(o, u0, u1, reinterpret_cast<__nv_bfloat16*>(p.out_s0), p.ld_s, static_cast<int64_t>(b) * p.Lq, p.Lq, h, p.hd, row0, t);
 #pragma unroll
-                for (int cc = 0; cc < 2; ++cc) {
-                    uint32_t(&v)[32] = cc ? vb : va;
-                    uint32_t pk[16];
-#pragma unroll
-                    for (int q = 0; q < 4; ++q) {
-                        float e[8];
-#pragma unroll
-                        for (int k = 0; k < 8; ++k) {
-                            const float arg = __uint_as_float(v[q * 8 + k]) * sc - m_new;
-                            if constexpr (kFull) {
-                                // IMAGD_ATTN_POLY of every 8 exponentials go to the FMA pipe instead of MUFU (default 0)
-                                e[k] = (k < IMAGD_ATTN_POLY) ? ex2_poly(arg) : ex2_approx(arg);
-                            } else {
-                                e[k] = (cc * 32 + q * 8 + k < valid) ? ex2_approx(arg) : 0.f;
-                            }
-                        }
-                        if constexpr (!kOnes) {
-                            sum0 += e[0] + e[4];
-                            sum1 += e[1] + e[5];
-                            sum2 += e[2] + e[6];
-                            sum3 += e[3] + e[7];
-                        }
-                        if constexpr (PT) {
-                            pk[q * 4 + 0] = pack_bf16x2(e[0], e[1]);
-                            pk[q * 4 + 1] = pack_bf16x2(e[2], e[3]);
-                            pk[q * 4 + 2] = pack_bf16x2(e[4], e[5]);
-                            pk[q * 4 + 3] = pack_bf16x2(e[6], e[7]);
-                        } else {
-                            const uint32_t chunk = static_cast<uint32_t>(cc * 4 + q) ^ rx;
-                            asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(p_row + chunk * 16),
-                                         "r"(pack_bf16x2(e[0], e[1])), "r"(pack_bf16x2(e[2], e[3])),
-                                         "r"(pack_bf16x2(e[4], e[5])), "r"(pack_bf16x2(e[6], e[7]))
-                                         : "memory");
-                        }
-                    }
-                    // 16 packed columns per 32 scores: the first store is in flight while the second half is computed
-                    if constexpr (PT) tmem_st16(tmem_S + lane_addr + half * 32 + cc * 16, pk);
-                }
-            };
-            if (full) {
-                pass2(std::true_type{});
-            } else {
-                pass2(std::false_type{});
-            }
-            if constexpr (!kOnes) l_run = l_run * alpha + ((sum0 + sum1) + (sum2 + sum3));
-
-            if constexpr (PT) {
-                tmem_st_wait();
-            } else {
-                fence_proxy_async_smem();  // generic-proxy P writes -> visible to the tensor core (async proxy)
-            }
-            tc_fence_before();
-            mbar_arrive(p_full);
+            for (int n = 0; n < NT; ++n) o[n][0] = o[n][1] = o[n][2] = o[n][3] = 0.f;
+            m_run[0] = m_run[1] = -INFINITY;
+            l_run[0] = l_run[1] = 0.f;
         }
+        cp_async_wait<0>();
+        __syncthreads();  // block i landed for every thread; every warp is done with block i - 1's stage
+        if (i + 1 < T) load_kv(i + 1);
+        cp_async_commit();
 
-        // ---- epilogue: out = w0 * O0 / l0 + w1 * O1 / l1 (row sums of the two half-row threads meet in the idle P tile)
-        mbar_wait(o_full, 0);
-        tc_fence_after();
-        float lf, lr;  // row sums of the first stream / the last stream
-        if constexpr (kOnes) {
-            uint32_t t0[16], t1[16];
-            tmem_ld16(tmem_O + lane_addr + 32, t0);  // columns 32..47 of O_0: element 8 is column 40
-            tmem_ld16(tmem_O + C::kOStride + lane_addr + 32, t1);
-            tmem_ld_wait();
-            lf = __uint_as_float(t0[8]);
-            lr = nb1 > 0 ? __uint_as_float(t1[8]) : lf;
-        } else {
-            float* lbuf = reinterpret_cast<float*>(sP);  // [2 halves][2 values][128 rows]
-            lbuf[(half * 2 + 0) * 128 + r] = l_first;
-            lbuf[(half * 2 + 1) * 128 + r] = l_run;
-            asm volatile("bar.sync %0, 64;" ::"r"(1 + lg) : "memory");
-            lf = l_first + lbuf[((half ^ 1) * 2 + 0) * 128 + r];
-            lr = l_run + lbuf[((half ^ 1) * 2 + 1) * 128 + r];
-        }
-        float w0, w1 = 0.f;
-        if (nb1 > 0) {
-            w0 = p.oscale0 / lf;
-            w1 = p.oscale1 / lr;
-        } else {
-            w0 = p.oscale0 / lr;
-        }
-        const int q = q0 + r;
-        __nv_bfloat16* orow =
-            reinterpret_cast<__nv_bfloat16*>(p.out) + (static_cast<int64_t>(b) * p.Lq + q) * p.out_ld + h * p.hd;
-        if (p.lse != nullptr && half == 0 && q < p.Lq) {  // training: log2-domain log-sum-exp per stream (m + log2 l)
-            const int64_t per = static_cast<int64_t>(p.heads) * p.lq_pad;
-            float* l0p = p.lse + (static_cast<int64_t>(b) * p.heads + h) * p.lq_pad + q;
-            if (nb1 > 0) {
-                l0p[0] = m_first + __log2f(lf);
-                l0p[static_cast<int64_t>(p.B) * per] = m_run + __log2f(lr);
-            } else {
-                l0p[0] = m_run + __log2f(lr);
+        // S = Q K^T: 16 rows x 64 keys per warp
+        float sc[8][4];
+#pragma unroll
+        for (int n = 0; n < 8; ++n) sc[n][0] = sc[n][1] = sc[n][2] = sc[n][3] = 0.f;
+        const uint32_t kb = sK + (i & 1) * C::kKVBytes;
+#pragma unroll
+        for (int ks = 0; ks < HDP / 16; ++ks) {
+            uint32_t a[4];
+            ldmatrix_x4(a, sQ + (warp * 16 + (lane & 15)) * kRow + (ks * 16 + (lane >> 4) * 8) * 2);
+#pragma unroll
+            for (int np = 0; np < 4; ++np) {
+                uint32_t bb[4];
+                ldmatrix_x4(bb, kb + (np * 16 + (lane & 7) + (lane >> 4) * 8) * kRow + (ks * 16 + ((lane >> 3) & 1) * 8) * 2);
+                mma_bf16_16816(sc[2 * np], a, bb[0], bb[1]);
+                mma_bf16_16816(sc[2 * np + 1], a, bb[2], bb[3]);
             }
         }
-        const bool per_stream = p.out_s0 != nullptr && nb1 > 0;  // training, two streams: O_s / l_s on their own
-        const float u0 = nb1 > 0 ? 1.f / lf : 0.f, u1 = nb1 > 0 ? 1.f / lr : 0.f;
-        const int64_t srow = (static_cast<int64_t>(b) * p.Lq + q) * p.ld_s + h * p.hd;
-#pragma unroll 1
-        for (int cc = ch_begin; cc < ch_end; ++cc) {
-            const int c = cc * 16;
-            uint32_t o0[16], o1[16];
-            tmem_ld16(tmem_O + lane_addr + c, o0);
-            if (nb1 > 0) tmem_ld16(tmem_O + C::kOStride + lane_addr + c, o1);
-            tmem_ld_wait();
-            if (q < p.Lq && c < p.hd) {
-                float f[16];
+        // mask + block row max (the four threads of a quad share a row)
+        const int len = p.kv[s].len;
+        float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
-                for (int k = 0; k < 16; ++k) {
-                    f[k] = w0 * __uint_as_float(o0[k]);
-                    if (nb1 > 0) f[k] += w1 * __uint_as_float(o1[k]);
-                }
-                uint4* dst = reinterpret_cast<uint4*>(orow + c);
-                dst[0] = make_uint4(pack_bf16x2(f[0], f[1]), pack_bf16x2(f[2], f[3]), pack_bf16x2(f[4], f[5]),
-                                    pack_bf16x2(f[6], f[7]));
-                if (c + 8 < p.hd)
-                    dst[1] = make_uint4(pack_bf16x2(f[8], f[9]), pack_bf16x2(f[10], f[11]), pack_bf16x2(f[12], f[13]),
-                                        pack_bf16x2(f[14], f[15]));
-                if (per_stream) {
+        for (int n = 0; n < 8; ++n) {
 #pragma unroll
-                    for (int st = 0; st < 2; ++st) {
-                        const uint32_t(&o)[16] = st ? o1 : o0;
-                        const float u = st ? u1 : u0;
-                        uint4* d2 = reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(st ? p.out_s1 : p.out_s0) + srow + c);
-                        d2[0] = make_uint4(pack_bf16x2(u * __uint_as_float(o[0]), u * __uint_as_float(o[1])),
-                                           pack_bf16x2(u * __uint_as_float(o[2]), u * __uint_as_float(o[3])),
-                                           pack_bf16x2(u * __uint_as_float(o[4]), u * __uint_as_float(o[5])),
-                                           pack_bf16x2(u * __uint_as_float(o[6]), u * __uint_as_float(o[7])));
-                        if (c + 8 < p.hd)
-                            d2[1] = make_uint4(pack_bf16x2(u * __uint_as_float(o[8]), u * __uint_as_float(o[9])),
-                                               pack_bf16x2(u * __uint_as_float(o[10]), u * __uint_as_float(o[11])),
-                                               pack_bf16x2(u * __uint_as_float(o[12]), u * __uint_as_float(o[13])),
-                                               pack_bf16x2(u * __uint_as_float(o[14]), u * __uint_as_float(o[15])));
-                    }
-                }
+            for (int e = 0; e < 4; ++e) {
+                const int key = j * 64 + n * 8 + 2 * t + (e & 1);
+                const int qrow = row0 + (e >> 1) * 8;
+                bool ok = key < len;
+                if (s == 0 && p.causal) ok = ok && key <= qrow;
+                sc[n][e] = ok ? sc[n][e] * p.scale_log2 : -INFINITY;
+                mx[e >> 1] = fmaxf(mx[e >> 1], sc[n][e]);
+            }
+        }
+        float alpha[2];
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+            const float m_new = fmaxf(m_run[hr], quad_max(mx[hr]));
+            alpha[hr] = ex2_approx(m_run[hr] - m_new);  // 0 on a stream's first block
+            m_run[hr] = m_new;
+            l_run[hr] *= alpha[hr];
+        }
+#pragma unroll
+        for (int n = 0; n < NT; ++n) {
+            o[n][0] *= alpha[0];
+            o[n][1] *= alpha[0];
+            o[n][2] *= alpha[1];
+            o[n][3] *= alpha[1];
+        }
+        // P = exp2(S - m) -> bf16 A fragments (keys 16 kk .. 16 kk + 15), O += P V
+        const uint32_t vb = sV + (i & 1) * C::kKVBytes;
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {
+            uint32_t a[4];
+#pragma unroll
+            for (int hf = 0; hf < 2; ++hf) {
+                float* c = sc[2 * kk + hf];
+                const float e0 = ex2_approx(c[0] - m_run[0]), e1 = ex2_approx(c[1] - m_run[0]);
+                const float e2 = ex2_approx(c[2] - m_run[1]), e3 = ex2_approx(c[3] - m_run[1]);
+                l_run[0] += e0 + e1;
+                l_run[1] += e2 + e3;
+                a[2 * hf] = pack_bf16x2(e0, e1);
+                a[2 * hf + 1] = pack_bf16x2(e2, e3);
+            }
+#pragma unroll
+            for (int np = 0; np < NT / 2; ++np) {
+                uint32_t bb[4];
+                ldmatrix_x4_trans(bb, vb + (kk * 16 + (lane & 7) + ((lane >> 3) & 1) * 8) * kRow + (np * 16 + (lane >> 4) * 8) * 2);
+                mma_bf16_16816(o[2 * np], a, bb[0], bb[1]);
+                mma_bf16_16816(o[2 * np + 1], a, bb[2], bb[3]);
             }
         }
     }
 
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 9) tmem_dealloc(tmem_base, C::kTmemCols);
+    // ---- epilogue: out = w0 * O0 / l0 + w1 * O1 / l1
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) l_run[hr] = quad_sum(l_run[hr]);
+    const float u0 = 1.f / l_run[0], u1 = 1.f / l_run[1];
+    if (p.lse != nullptr && t == 0) {  // training: log2-domain log-sum-exp per stream (m + log2 l)
+        const int64_t per = static_cast<int64_t>(p.B) * p.heads * p.lq_pad;
+        float* lp = p.lse + (static_cast<int64_t>(b) * p.heads + h) * p.lq_pad;
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+            const int q = row0 + hr * 8;
+            if (q >= p.Lq) continue;
+            if (nb1 > 0) {
+                lp[q] = m_first[hr] + __log2f(l_first[hr]);
+                lp[per + q] = m_run[hr] + __log2f(l_run[hr]);
+            } else {
+                lp[q] = m_run[hr] + __log2f(l_run[hr]);
+            }
+        }
+    }
+    if (nb1 > 0 && p.out_s1 != nullptr)
+        attn_store_frag<NT>(o, u0, u1, reinterpret_cast<__nv_bfloat16*>(p.out_s1), p.ld_s, static_cast<int64_t>(b) * p.Lq, p.Lq, h, p.hd, row0, t);
+    const float w = nb1 > 0 ? p.oscale1 : p.oscale0;
+#pragma unroll
+    for (int n = 0; n < NT; ++n) {
+        float f[4] = {w * o[n][0] * u0, w * o[n][1] * u0, w * o[n][2] * u1, w * o[n][3] * u1};
+        if (nb1 > 0) {
+#pragma unroll
+            for (int e = 0; e < 4; ++e) f[e] += s_out[(n * 4 + e) * 256 + threadIdx.x];
+        }
+        o[n][0] = f[0];
+        o[n][1] = f[1];
+        o[n][2] = f[2];
+        o[n][3] = f[3];
+    }
+    attn_store_frag<NT>(o, 1.f, 1.f, reinterpret_cast<__nv_bfloat16*>(p.out), p.out_ld, static_cast<int64_t>(b) * p.Lq, p.Lq, h, p.hd, row0, t);
 }
-
-#include "attention_pp.inc"
-#include "attention_pp1.inc"
-#include "attention_pp3.inc"
 
 // ------------------------------------------------------------------------------------------------ host side
 
-static int make_head_tmap(CUtensorMap* tm, const void* base, int64_t ld, int hd, int heads, int len, int nsamples,
-                          int sample_rows = 0, int box_rows = 128) {
-    uint64_t dims[4] = {static_cast<uint64_t>(hd), static_cast<uint64_t>(heads), static_cast<uint64_t>(len),
-                        static_cast<uint64_t>(nsamples)};
-    uint64_t strides[3] = {static_cast<uint64_t>(hd) * 2, static_cast<uint64_t>(ld) * 2,
-                           static_cast<uint64_t>(ld) * 2 * (sample_rows > 0 ? sample_rows : len)};
-    uint32_t box[4] = {64, 1, static_cast<uint32_t>(box_rows), 1};
-    return make_tmap_bf16(tm, base, 4, dims, strides, box);
-}
-
-template <int HD_MMA, int NATOM, int KV_STAGES, bool PT>
-static int launch_attn(const CUtensorMap* tms, const AttnParams& p, cudaStream_t stream) {
-    using C = AttnCfg<HD_MMA, NATOM, KV_STAGES, PT>;
-    IMAGD_SET_MAX_SMEM((attention_tc_kernel<HD_MMA, NATOM, KV_STAGES, PT>), C::kTotal);
+template <int HDP>
+static int launch_attn(const AttnParams& p, cudaStream_t stream) {
+    using C = AttnSmem<HDP>;
+    IMAGD_SET_MAX_SMEM(attention_fwd_kernel<HDP>, C::kTotal);
     dim3 grid((p.Lq + 127) / 128, p.heads, p.B);
-    IMAGD_CUDA(launch_pdl(attention_tc_kernel<HD_MMA, NATOM, KV_STAGES, PT>, grid, dim3(320), C::kTotal, stream, tms[0],
-                          tms[1], tms[2], tms[3], tms[4], p));
+    IMAGD_CUDA(launch_pdl(attention_fwd_kernel<HDP>, grid, dim3(256), C::kTotal, stream, p));
     return IMAGD_OK;
-}
-
-static int env_int(const char* name, int dflt) {
-    const char* e = getenv(name);
-    return e ? atoi(e) : dflt;
-}
-
-// IMAGD_ATTN_PP_VARIANT: 1 = P aliases S (first build), 2 = separate P buffer, 3 = one thread per row, 64-key blocks,
-// double-buffered S (its K / V tensor maps fetch 64-row boxes)
-static int attn_pp_variant() {
-    static const int v = env_int("IMAGD_ATTN_PP_VARIANT", 1);
-    return v;
-}
-
-template <int HD_MMA>
-static int launch_attn_pp3(const CUtensorMap* tms, AttnParams p, cudaStream_t stream) {
-    constexpr int kStages = 6;
-    using C = AttnPP3Cfg<kStages>;
-    static const int sync = env_int("IMAGD_ATTN_PP_SYNC", 1);
-    p.pp_sync = sync;
-    dim3 grid((p.Lq + 255) / 256, p.heads, p.B);
-    IMAGD_SET_MAX_SMEM((attention_pp3_kernel<HD_MMA, kStages>), C::kTotal);
-    IMAGD_CUDA(launch_pdl(attention_pp3_kernel<HD_MMA, kStages>, grid, dim3(320), C::kTotal, stream, tms[0], tms[1], tms[2],
-                          tms[3], tms[4], p));
-    return IMAGD_OK;
-}
-
-template <int HD_MMA>
-static int launch_attn_pp(const CUtensorMap* tms, AttnParams p, cudaStream_t stream) {
-    constexpr int kStages = 3;
-    // A/B switches (read once): IMAGD_ATTN_PP_VARIANT = 1 (P aliases S; default) | 2 (separate P buffer, early S(i+1));
-    // IMAGD_ATTN_PP_SYNC = 1 (strict hand-over of the MUFU pipe between the groups; default) | 0 (free-running groups).
-    // Measured on B200, level-0 hybrid attention, batch 1 / 8 (profiles/r02_call5_attention_matrix_clip.txt):
-    //   variant 1 sync 1: 197.9 / 1202.8 us   variant 1 sync 0: 216.0 / 1260.0 us
-    //   variant 2 sync 1: 221.7 / 1347.5 us   variant 2 sync 0: 212.0 / 1321.5 us   two-CTAs-per-SM kernel: 214 / 1298 us
-    static const int variant = attn_pp_variant();
-    static const int sync = env_int("IMAGD_ATTN_PP_SYNC", 1);
-    p.pp_sync = sync;
-    static const int spin = env_int("IMAGD_ATTN_SPIN", 0);
-    p.spin = spin;
-    dim3 grid((p.Lq + 255) / 256, p.heads, p.B);
-    if (variant == 1) {
-        using C = AttnPP1Cfg<kStages>;
-        static const int poly = env_int("IMAGD_ATTN_POLY", IMAGD_ATTN_POLY);  // exponentials per 8 on the FMA pipe
-        static const int pack = env_int("IMAGD_ATTN_PACK", 0);                // bf16 packing of P: 0 F2FP, 1 truncate, 2 round + permute
-#define IMAGD_PP1_LAUNCH(P, K)                                                                                           \
-    do {                                                                                                                 \
-        IMAGD_SET_MAX_SMEM((attention_pp1_kernel<HD_MMA, kStages, P, K>), C::kTotal);                                    \
-        IMAGD_CUDA(launch_pdl(attention_pp1_kernel<HD_MMA, kStages, P, K>, grid, dim3(576), C::kTotal, stream, tms[0],   \
-                              tms[1], tms[2], tms[3], tms[4], p));                                                       \
-        return IMAGD_OK;                                                                                                 \
-    } while (0)
-        if (pack == 1) {
-            if (poly == 2) IMAGD_PP1_LAUNCH(2, 1);
-            IMAGD_PP1_LAUNCH(0, 1);
-        }
-        if (pack == 2) {
-            if (poly == 2) IMAGD_PP1_LAUNCH(2, 2);
-            IMAGD_PP1_LAUNCH(0, 2);
-        }
-        switch (poly) {
-            case 1: IMAGD_PP1_LAUNCH(1, 0);
-            case 2: IMAGD_PP1_LAUNCH(2, 0);
-            case 3: IMAGD_PP1_LAUNCH(3, 0);
-            case 4: IMAGD_PP1_LAUNCH(4, 0);
-            default: IMAGD_PP1_LAUNCH(0, 0);
-        }
-#undef IMAGD_PP1_LAUNCH
-    }
-    using C = AttnPPCfg<kStages>;
-    IMAGD_SET_MAX_SMEM((attention_pp_kernel<HD_MMA, kStages>), C::kTotal);
-    IMAGD_CUDA(launch_pdl(attention_pp_kernel<HD_MMA, kStages>, grid, dim3(576), C::kTotal, stream, tms[0], tms[1], tms[2],
-                          tms[3], tms[4], p));
-    return IMAGD_OK;
-}
-
-// IMAGD_ATTN_PP=0 switches the ping-pong kernel (two Q tiles per CTA, head_dim 40 / 64, Lq > 128) off (A/B switch).
-static bool attn_pp() {
-    static const bool on = [] {
-        const char* e = getenv("IMAGD_ATTN_PP");
-        return e == nullptr || e[0] != '0';
-    }();
-    return on;
-}
-
-// IMAGD_ATTN_PTMEM=0 falls back to the shared-memory P path of round 1 (A/B switch; read once).
-static bool attn_ptmem() {
-    static const bool on = [] {
-        const char* e = getenv("IMAGD_ATTN_PTMEM");
-        return e == nullptr || e[0] != '0';
-    }();
-    return on;
 }
 
 }  // namespace imagd
@@ -660,23 +281,29 @@ static int attention_impl(const void* q, int64_t q_ld, void* out, int64_t out_ld
     IMAGD_CHECK_ARG(s0->sample_rows == 0 || s0->sample_rows >= s0->len, "attention: sample_rows < len");
     const bool has1 = s1 != nullptr && s1->k != nullptr && s1->len > 0 && s1->n_query_samples > 0;
 
-    AttnParams p;
+    AttnParams p{};
     p.B = B;
     p.Lq = Lq;
     p.heads = heads;
     p.hd = head_dim;
     p.scale_log2 = sm_scale * 1.4426950408889634f;
-    p.len0 = s0->len;
-    p.bcast0 = s0->broadcast;
-    p.oscale0 = s0->out_scale;
-    p.len1 = has1 ? s1->len : 0;
+    p.q = static_cast<const __nv_bfloat16*>(q);
+    p.q_ld = q_ld;
+    const imagd_kv_stream* ss[2] = {s0, has1 ? s1 : s0};
+    for (int s = 0; s < 2; ++s) {
+        p.kv[s].k = static_cast<const __nv_bfloat16*>(ss[s]->k);
+        p.kv[s].v = static_cast<const __nv_bfloat16*>(ss[s]->v);
+        p.kv[s].ld = ss[s]->ld;
+        p.kv[s].len = ss[s]->len;
+        p.kv[s].sample_rows = ss[s]->sample_rows > 0 ? ss[s]->sample_rows : ss[s]->len;
+        p.kv[s].bcast = ss[s]->broadcast;
+        IMAGD_CHECK_ARG(ss[s]->ld % 8 == 0 && aligned16(ss[s]->k) && aligned16(ss[s]->v), "attention: K / V alignment");
+    }
+    IMAGD_CHECK_ARG(q_ld % 8 == 0 && aligned16(q), "attention: Q alignment");
     p.nq1 = has1 ? (s1->n_query_samples < B ? s1->n_query_samples : B) : 0;
-    p.bcast1 = has1 ? s1->broadcast : 0;
+    p.oscale0 = s0->out_scale;
     p.oscale1 = has1 ? s1->out_scale : 0.f;
     p.causal = causal;
-    p.pp_sync = 1;
-    p.spin = 0;
-    p.pdl_late = pdl_mode() == 2 ? 1 : 0;
     p.out = out;
     p.out_ld = out_ld;
     p.lse = aux ? aux->lse : nullptr;
@@ -691,53 +318,11 @@ static int attention_impl(const void* q, int64_t q_ld, void* out, int64_t out_ld
                         "attention(train): two streams need out_s0 / out_s1");
         IMAGD_CHECK_ARG(!causal, "attention(train): causal not supported");
     }
-
-    CUtensorMap tms[5];
-    int rc = make_head_tmap(&tms[0], q, q_ld, head_dim, heads, Lq, B);
-    if (rc != IMAGD_OK) return rc;
-    rc = make_head_tmap(&tms[1], s0->k, s0->ld, head_dim, heads, s0->len, s0->broadcast ? 1 : B, s0->sample_rows);
-    if (rc != IMAGD_OK) return rc;
-    rc = make_head_tmap(&tms[2], s0->v, s0->ld, head_dim, heads, s0->len, s0->broadcast ? 1 : B, s0->sample_rows);
-    if (rc != IMAGD_OK) return rc;
-    if (has1) {
-        const int ns = s1->broadcast ? 1 : p.nq1;
-        rc = make_head_tmap(&tms[3], s1->k, s1->ld, head_dim, heads, s1->len, ns, s1->sample_rows);
-        if (rc != IMAGD_OK) return rc;
-        rc = make_head_tmap(&tms[4], s1->v, s1->ld, head_dim, heads, s1->len, ns, s1->sample_rows);
-        if (rc != IMAGD_OK) return rc;
-    } else {
-        tms[3] = tms[1];
-        tms[4] = tms[2];
-    }
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    // the training-mode outputs (lse / per-stream O) exist in the first ping-pong build and in the two-CTAs-per-SM kernel;
-    // IMAGD_ATTN_TRAIN_PP=0 keeps training forwards on the latter (A/B)
-    static const int train_pp = env_int("IMAGD_ATTN_TRAIN_PP", 1);
-    const bool pp_ok = !aux || (train_pp && attn_pp_variant() == 1);
-    if (attn_pp() && pp_ok && !causal && Lq > 128 && (head_dim == 40 || head_dim == 64)) {
-        if (attn_pp_variant() == 3) {  // K / V through 64-row boxes
-            rc = make_head_tmap(&tms[1], s0->k, s0->ld, head_dim, heads, s0->len, s0->broadcast ? 1 : B, s0->sample_rows, 64);
-            if (rc != IMAGD_OK) return rc;
-            rc = make_head_tmap(&tms[2], s0->v, s0->ld, head_dim, heads, s0->len, s0->broadcast ? 1 : B, s0->sample_rows, 64);
-            if (rc != IMAGD_OK) return rc;
-            if (has1) {
-                const int ns = s1->broadcast ? 1 : p.nq1;
-                rc = make_head_tmap(&tms[3], s1->k, s1->ld, head_dim, heads, s1->len, ns, s1->sample_rows, 64);
-                if (rc != IMAGD_OK) return rc;
-                rc = make_head_tmap(&tms[4], s1->v, s1->ld, head_dim, heads, s1->len, ns, s1->sample_rows, 64);
-                if (rc != IMAGD_OK) return rc;
-            } else {
-                tms[3] = tms[1];
-                tms[4] = tms[2];
-            }
-            return head_dim == 40 ? launch_attn_pp3<48>(tms, p, st) : launch_attn_pp3<64>(tms, p, st);
-        }
-        return head_dim == 40 ? launch_attn_pp<48>(tms, p, st) : launch_attn_pp<64>(tms, p, st);
-    }
     switch (head_dim) {
-        case 40: return attn_ptmem() ? launch_attn<48, 1, 2, true>(tms, p, st) : launch_attn<48, 1, 2, false>(tms, p, st);
-        case 64: return attn_ptmem() ? launch_attn<64, 1, 2, true>(tms, p, st) : launch_attn<64, 1, 2, false>(tms, p, st);
-        case 80: return launch_attn<80, 2, 2, false>(tms, p, st);
-        default: return launch_attn<160, 3, 1, false>(tms, p, st);
+        case 40: return launch_attn<48>(p, st);
+        case 64: return launch_attn<64>(p, st);
+        case 80: return launch_attn<80>(p, st);
+        default: return launch_attn<160>(p, st);
     }
 }

@@ -12,6 +12,8 @@
 
 namespace imagd {
 
+constexpr int kNumSms = 132;  // H100 SXM: grid caps of the grid-stride / chunked kernels
+
 void set_error(const char* fmt, ...);
 int cuda_fail(cudaError_t e, const char* what);
 

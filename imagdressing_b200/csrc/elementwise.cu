@@ -88,8 +88,8 @@ __global__ void im2col3x3_s2_kernel(const __nv_bfloat16* __restrict__ x, __nv_bf
 // Row softmax of an fp32 score matrix into bf16 probabilities: P[r, :] = softmax(scale * S[r, :]). One CTA per row, the
 // row lives in registers (<= 64 values per thread = 16384 columns), fp32 statistics, fixed-order block reductions. Serves
 // the single-head, head-dim-512 attention of the VAE mid block (AutoencoderKL, diffusers-0.24: 4096..6912 tokens at
-// 512x512..768x576), whose 512-wide head does not fit the TMEM budget of the flash kernel: S = Q K^T and O = P V run as
-// plain tcgen05 GEMMs around this HBM-bound pass (2 x rows x cols x 4 B read, 2 B written per element).
+// 512x512..768x576), whose 512-wide head does not fit the register budget of the flash kernel: S = Q K^T and O = P V run
+// as plain GEMMs around this HBM-bound pass (2 x rows x cols x 4 B read, 2 B written per element).
 __global__ void __launch_bounds__(256) softmax_rows_kernel(const float* __restrict__ s, int64_t lds,
                                                            __nv_bfloat16* __restrict__ p, int64_t ldp, int cols,
                                                            float scale_log2) {
@@ -479,7 +479,7 @@ __global__ void cfg_ddim_step_kernel(const float* __restrict__ eps_c, const floa
 
 static inline int grid_for(int64_t total, int threads) {
     int64_t g = (total + threads - 1) / threads;
-    if (g > 148 * 16) g = 148 * 16;
+    if (g > kNumSms * 16) g = kNumSms * 16;
     if (g < 1) g = 1;
     return static_cast<int>(g);
 }
@@ -599,7 +599,7 @@ int imagd_conv3x3_direct_bf16(const void* x, int NB, int H, int W, int Cin, cons
     }
     const int Ho = (H + stride - 1) / stride, Wo = (W + stride - 1) / stride;
     const int64_t total = static_cast<int64_t>(NB) * Ho * Wo * Cout;
-    const int tgrid = std::min(grid_for(total, 256) * 4, 148 * 64);
+    const int tgrid = std::min(grid_for(total, 256) * 4, kNumSms * 64);
     IMAGD_CUDA(launch_pdl(conv3x3_direct_thread_kernel, dim3(tgrid), dim3(256), 0, st, reinterpret_cast<const __nv_bfloat16*>(x), NB, H, W, Cin,
                                          reinterpret_cast<const __nv_bfloat16*>(w), bias, y, Cout, stride, act,
                                          out_nchw_f32, reinterpret_cast<const __nv_bfloat16*>(add_nhwc)));
@@ -643,7 +643,7 @@ int imagd_cfg_ddim_step(const float* eps_cond, const float* eps_uncond, float gu
     IMAGD_CHECK_ARG(!mask || (image_latents && noise && blend_coef), "cfg_ddim_step: inpaint blend needs all operands");
     const int64_t total = static_cast<int64_t>(NB) * C * HW;
     int grid = grid_for(total, 256);
-    if (grid > 148) grid = 148;
+    if (grid > kNumSms) grid = kNumSms;
     IMAGD_CUDA(launch_pdl(cfg_ddim_step_kernel, dim3(grid), dim3(256), 0, static_cast<cudaStream_t>(stream), 
         eps_cond, eps_uncond, guidance, latents, coef, step_ptr, mask, image_latents, noise, blend_coef, NB, C, HW));
     return IMAGD_OK;

@@ -1,4 +1,4 @@
-// tcgen05 GEMM / implicit-GEMM 3x3 convolution for sm_100a.
+// wgmma GEMM / implicit-GEMM 3x3 convolution for sm_90a.
 //
 //   D[p, c] = epilogue( sum_{tap, k} A_tap[p, k] * W[c, tap*Cin + k] )
 //
@@ -7,11 +7,10 @@
 // hardware zero-fills — that is the conv's zero padding, with no im2col buffer. A plain GEMM is the same
 // kernel with one tap and a [K, M, 1, 1] view.
 //
-// CTA = 128 output pixels x BLOCK_N output channels. Warp roles (192 threads):
-//   warp 0     TMA producer   (one elected lane; STAGES-deep smem ring, full/empty mbarriers)
-//   warp 1     TMEM allocator + tcgen05.mma issuer (one elected lane; fp32 accumulator in TMEM)
-//   warps 2-5  epilogue: tcgen05.ld -> bias / time-embedding row vector / activation / residual -> bf16 stores
-// Two CTAs fit per SM (96 KB smem, <=128 TMEM columns each) so one CTA's epilogue overlaps the other's mainloop.
+// CTA = 128 output pixels x BLOCK_N output channels: a TMA producer warp feeds a STAGES-deep ring of 128B-swizzled
+// A / B tiles, two warpgroups accumulate 64 rows each with wgmma in registers, and the accumulator tile is handed to
+// the epilogue through shared memory (bias / time-embedding row vector / activation / residual -> bf16 stores).
+// One CTA runs per SM (288 threads, up to 168 registers each, 96-200 KB of shared memory).
 #include <algorithm>
 #include <cstring>
 #include <mutex>
@@ -45,9 +44,6 @@ struct GemmParams {
     unsigned int* counters;
     // debug: when non-null, every CTA records its timeline (imagd_gemm_debug_timeline; tools/gemm_timeline.py)
     unsigned long long* dbg;
-    // persistent kernel (gemm_persist.inc): N tiles per M tile row and total tile count
-    int persist_n_tiles;
-    int persist_total;
     int ups_n_tiles;  // LNM == 3: N tiles per phase (gridDim.y = 4 * ups_n_tiles)
     int pdl_late;     // 1: release the dependent kernel when the accumulator is complete instead of at kernel entry
 };
@@ -62,57 +58,54 @@ __device__ __forceinline__ void dbg_mark(const GemmParams& p, int slot) {
 constexpr int kBlockM = 128;
 constexpr int kBlockK = 64;
 constexpr int kABytes = kBlockM * kBlockK * 2;  // 16 KB
+constexpr int kGemmThreads = 288;               // two consumer warpgroups + one producer warp
 
 template <int BLOCK_N, int STAGES>
 struct GemmSmem {
     static constexpr int kBBytes = BLOCK_N * kBlockK * 2;
     static constexpr int kStageBytes = kABytes + kBBytes;
-    static constexpr int kBarOffset = STAGES * kStageBytes;
-    static constexpr int kVecOffset = (kBarOffset + (2 * STAGES + 1) * 8 + 16 + 15) & ~15;  // float4 reads
+    static constexpr int kRing = STAGES * kStageBytes;
+    // after the mainloop the fp32 accumulator tile is staged row by row over the idle operand ring: one row per epilogue
+    // thread, +16 bytes so that the float4 reads of eight consecutive rows hit eight bank groups
+    static constexpr int kAccRowBytes = BLOCK_N * 4 + 16;
+    static constexpr int kAccBytes = kBlockM * kAccRowBytes;
+    static constexpr int kBarOffset = (kRing > kAccBytes ? kRing : kAccBytes);
+    static constexpr int kVecOffset = (kBarOffset + (2 * STAGES) * 8 + 16 + 15) & ~15;  // float4 reads
     // epilogue vectors staged once per CTA: bias[BLOCK_N] | row vector[BLOCK_N] (when the tile lies in one row group)
     static constexpr int kTotal = kVecOffset + 2 * BLOCK_N * 4;
-    // EPI 3 only: four mbarriers (one per epilogue warp) for the bulk-loaded residual rows, after the vectors
-    static constexpr int kResBarOffset = kTotal;  // 16-byte aligned: BLOCK_N * 8 is a multiple of 16
-    static constexpr int kTotalRes = kTotal + 4 * 8;
 };
 
-__host__ __device__ constexpr int tmem_cols_for(int n) { return n <= 64 ? 64 : (n <= 128 ? 128 : 256); }
-
 // LINEAR = the epilogue has no activation and writes bf16 (every conv and most linears of the UNet): straight-line,
-// branch-free column loop with the next TMEM chunk and the next residual chunk in flight. !LINEAR = the generic epilogue
-// EPI 3 (r2-prep, never run): EPI 2 + the residual row arrives by ONE bulk copy into the same staging row (one exposed
-// round trip instead of a chain of per-chunk loads), is added from shared memory and overwritten in place by the output.
-// (SiLU / GELU / GEGLU / fp32 output). EPI: 0 generic, 1 LINEAR, 2 LINEAR with the output row staged in the (idle)
-// operand ring and written by one bulk copy per row instead of 16-byte stores (opt-in: IMAGD_GEMM_BULK_STORE=1;
-// written at the end of round 1, parity-tested but not yet tuned / made the default).
-// LNM: LayerNorm folding (r2-prep, see include/imagd_b200.h): 0 off, 1 producer (emit per-row {sum, sum of squares}
-// of the rounded outputs, one slot per N tile), 2 consumer (apply rstd * (alpha * acc - mean * colsum) + bias).
+// branch-free column loop. !LINEAR = the generic epilogue (SiLU / GELU / GEGLU / fp32 output).
+// EPI: 0 generic, 1 LINEAR, 2 LINEAR with the output row staged in shared memory (in the thread's own accumulator row,
+// behind the columns it has already read) and written by one bulk copy per row instead of 16-byte stores.
+// LNM: LayerNorm folding (see include/imagd_b200.h): 0 off, 1 producer (emit per-row {sum, sum of squares} of the rounded
+// outputs, one slot per N tile), 2 consumer (apply rstd * (alpha * acc - mean * colsum) + bias).
+//
+// CTA = 128 output pixels x BLOCK_N output channels, 288 threads:
+//   warps 0-3  warpgroup 0: wgmma on accumulator rows 0-63, then the epilogue (thread = tile row)
+//   warps 4-7  warpgroup 1: wgmma on accumulator rows 64-127
+//   warp 8     TMA producer (one elected lane; STAGES-deep smem ring, full / empty mbarriers)
 template <int BLOCK_N, int STAGES, int EPI, int LNM>
-__global__ void __launch_bounds__(192, (GemmSmem<BLOCK_N, STAGES>::kTotal <= 112 * 1024) ? 2 : 1)
+__global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
     using L = GemmSmem<BLOCK_N, STAGES>;
     constexpr bool LINEAR = EPI != 0;
-    constexpr bool BULK = EPI == 2 || EPI == 3;
-    constexpr bool BULK_RES = EPI == 3;
+    constexpr bool BULK = EPI == 2;
     constexpr bool LN_PRODUCE = LNM == 1;
     constexpr bool LN_CONSUME = LNM == 2;
-    // LNM == 3 (r2-prep, never run): nearest-2x upsample + 3x3 conv as four 2x2 "phase" convs on the LOW-resolution
-    // input (2.25x fewer MACs, no upsampled tensor): blockIdx.y = phase * n_tiles + n_blk, phase = py * 2 + px; tap
-    // t = ty * 2 + tx reads input pixel (y + py - 1 + ty, x + px - 1 + tx); the weight matrix is [4 * N, 4 * Cin]
-    // (phase-major rows, tap-major columns); output pixel (2y + py, 2x + px) of a [NB, 2H, 2W, N] tensor.
+    // LNM == 3: nearest-2x upsample + 3x3 conv as four 2x2 "phase" convs on the LOW-resolution input (2.25x fewer MACs,
+    // no upsampled tensor): blockIdx.y = phase * n_tiles + n_blk, phase = py * 2 + px; tap t = ty * 2 + tx reads input
+    // pixel (y + py - 1 + ty, x + px - 1 + tx); the weight matrix is [4 * N, 4 * Cin] (phase-major rows, tap-major
+    // columns); output pixel (2y + py, 2x + px) of a [NB, 2H, 2W, N] tensor.
     constexpr bool UPS = LNM == 3;
     static_assert(!LN_PRODUCE || LINEAR, "row statistics are emitted by the LINEAR epilogue only");
-    constexpr int kRowStage = BLOCK_N * 2 + 16;  // staged output row stride (bytes): +16 keeps 8 rows on 8 bank groups
-    static_assert(!BULK || 128 * kRowStage <= L::kBarOffset, "output staging must fit in the operand ring");
+    static_assert(BLOCK_N % 64 == 0 || BLOCK_N == 160, "wgmma N tile");
     extern __shared__ __align__(1024) uint8_t smem[];  // SWIZZLE_128B tiles need 1024-byte alignment
-    if (threadIdx.x == 0 && (smem_u32(smem) & 1023u) != 0) {
-        printf("imagd: dynamic shared memory base %u is not 1024-byte aligned\n", smem_u32(smem));
-        __trap();
-    }
+    if (threadIdx.x == 0 && (smem_u32(smem) & 1023u) != 0) __trap();  // (no printf: see mbar_wait_quiet)
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::kBarOffset);
     uint64_t* empty_bar = full_bar + STAGES;
-    uint64_t* tmem_full_bar = empty_bar + STAGES;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_full_bar + 1);
+    uint32_t* flag_slot = reinterpret_cast<uint32_t*>(empty_bar + STAGES);
     float* s_bias = reinterpret_cast<float*>(smem + L::kVecOffset);
     float* s_rowvec = s_bias + BLOCK_N;
 
@@ -147,33 +140,21 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         tma_prefetch_desc(&tmB);
         for (int i = 0; i < STAGES; ++i) {
             mbar_init(&full_bar[i], 1);
-            mbar_init(&empty_bar[i], 1);
-        }
-        mbar_init(tmem_full_bar, 1);
-        if constexpr (BULK_RES) {
-            uint64_t* res_bar = reinterpret_cast<uint64_t*>(smem + L::kResBarOffset);
-            for (int i = 0; i < 4; ++i) mbar_init(&res_bar[i], 1);
+            mbar_init(&empty_bar[i], 2);  // one arrival per consumer warpgroup
         }
         fence_barrier_init();
     }
-    if (warp == 1) {
-        tmem_alloc(tmem_slot, tmem_cols_for(BLOCK_N));
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     if (threadIdx.x == 0) dbg_mark(p, 1);
     pdl_wait();  // predecessor's output (our A operand / residual) and our output buffer are safe from here on
 
-    if (warp == 0) {
+    if (warp == 8) {
         if (elect_one()) {
             for (int i = 0; i < nk; ++i) {
                 const int kb = kb_begin + i;
                 const int stage = i % STAGES;
                 const uint32_t phase = (i / STAGES) & 1;
-                mbar_wait(&empty_bar[stage], phase ^ 1);
+                mbar_wait_quiet(&empty_bar[stage], phase ^ 1);
                 mbar_arrive_expect_tx(&full_bar[stage], L::kStageBytes);
                 const int tap = kb / p.kb_per_tap;
                 const int kc = kb - tap * p.kb_per_tap;
@@ -192,53 +173,26 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                             (UPS ? ups_phase * p.N : 0) + n_blk * BLOCK_N);
             }
         }
-    } else if (warp == 1) {
-        if (elect_one()) {
-            constexpr uint32_t idesc = umma_idesc_bf16(kBlockM, BLOCK_N, 0, 0);
-            for (int i = 0; i < nk; ++i) {
-                const int stage = i % STAGES;
-                const uint32_t phase = (i / STAGES) & 1;
-                mbar_wait(&full_bar[stage], phase);
-                tc_fence_after();
-                if (i == 0) dbg_mark(p, 2);
-                const uint32_t sa = smem_u32(smem + stage * L::kStageBytes);
-                const uint32_t sb = sa + kABytes;
-#pragma unroll
-                for (int k = 0; k < kBlockK / 16; ++k) {
-                    const uint64_t adesc = umma_smem_desc_sw128(sa + k * 32, 16, 1024);
-                    const uint64_t bdesc = umma_smem_desc_sw128(sb + k * 32, 16, 1024);
-                    umma_bf16(tmem_base, adesc, bdesc, idesc, (i | k) != 0 ? 1u : 0u);
-                }
-                umma_commit(&empty_bar[stage]);  // frees the smem slot when these MMAs retire
-            }
-            umma_commit(tmem_full_bar);  // accumulator complete
-            dbg_mark(p, 3);
-        }
-    } else {
-        // ---------------- epilogue ----------------
-        const int lane_group = warp & 3;               // TMEM lanes [32*lane_group, +32) belong to this warp
-        const int r = lane_group * 32 + lane;          // tile-local pixel
-        const int x = x0 + r % p.bw;
-        const int y = y0 + (r / p.bw) % p.bh;
-        const int n = n0 + r / (p.bw * p.bh);
-        const bool row_ok = (x < p.W) && (y < p.H) && (n < p.NB);
-        const int64_t pix = UPS ? (static_cast<int64_t>(n) * (2 * p.H) + (2 * y + (ups_phase >> 1))) * (2 * p.W) +
-                                      (2 * x + (ups_phase & 1))
-                                : (static_cast<int64_t>(n) * p.H + y) * p.W + x;
-        const imagd_epilogue& ep = p.ep;
-        const float alpha = ep.alpha;
-        const __nv_bfloat16* res = nullptr;
-        if (ep.residual != nullptr && row_ok)
-            res = reinterpret_cast<const __nv_bfloat16*>(ep.residual) + pix * ep.ldr;
-        const bool split = p.splits > 1;
+        return;
+    }
 
-        // ---- while the mainloop runs: stage the per-column vectors in shared memory (every row of the tile reads the
-        // same bias; the row vector too when the whole tile lies in one row group, i.e. one sample) and fetch the first
-        // residual chunk. Loads issued one at a time inside the column loop serialise on L2 latency (measured: the
-        // epilogue took 14-26k clocks vs 5-9k without bias / residual), so everything the loop needs is in flight early.
-        const int col_base = n_blk * BLOCK_N;
-        const float* rowvec = nullptr;   // per-thread global fallback (tile spans several row groups)
-        bool rowvec_shared = false;
+    const int wg = warp >> 2;  // consumer warpgroup: accumulator rows [64 wg, 64 wg + 64)
+    const imagd_epilogue& ep = p.ep;
+    const int col_base = n_blk * BLOCK_N;
+    // ---- epilogue preparation (warpgroup 0, before the mainloop): stage the per-column vectors in shared memory (every
+    // row of the tile reads the same bias; the row vector too when the whole tile lies in one row group, i.e. one sample)
+    const int r = threadIdx.x;  // warpgroup 0: tile-local pixel
+    const int x = x0 + r % p.bw;
+    const int y = y0 + (r / p.bw) % p.bh;
+    const int n = n0 + r / (p.bw * p.bh);
+    const bool row_ok = (x < p.W) && (y < p.H) && (n < p.NB);
+    const int64_t pix = UPS ? (static_cast<int64_t>(n) * (2 * p.H) + (2 * y + (ups_phase >> 1))) * (2 * p.W) +
+                                  (2 * x + (ups_phase & 1))
+                            : (static_cast<int64_t>(n) * p.H + y) * p.W + x;
+    const float* rowvec = nullptr;  // per-thread global fallback (tile spans several row groups)
+    bool rowvec_shared = false;
+    float ln_mean = 0.f, ln_rstd = 0.f;
+    if (wg == 0) {
         if (ep.rowvec != nullptr) {
             const int xl = min(x0 + p.bw, p.W) - 1, yl = min(y0 + p.bh, p.H) - 1, nl = min(n0 + p.bn, p.NB) - 1;
             const int64_t pix_first = (static_cast<int64_t>(n0) * p.H + y0) * p.W + x0;
@@ -247,35 +201,24 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             rowvec_shared = g_first == pix_last / ep.rows_per_group;
             if (rowvec_shared) {
                 const float* src = ep.rowvec + g_first * ep.rowvec_ld;
-                for (int c = threadIdx.x - 64; c < BLOCK_N; c += 128)
+                for (int c = threadIdx.x; c < BLOCK_N; c += 128)
                     s_rowvec[c] = (col_base + c < p.N) ? __ldg(src + col_base + c) : 0.f;
             } else if (row_ok) {
                 rowvec = ep.rowvec + (pix / ep.rows_per_group) * ep.rowvec_ld;
             }
         }
         if constexpr (LN_CONSUME) {  // the row-vector slot carries the folded weight's column sums instead
-            for (int c = threadIdx.x - 64; c < BLOCK_N; c += 128)
+            for (int c = threadIdx.x; c < BLOCK_N; c += 128)
                 s_rowvec[c] = (col_base + c < p.N) ? __ldg(ep.colsum + col_base + c) : 0.f;
         } else if (LINEAR && !rowvec_shared) {  // the straight-line loop always adds the staged vectors: absent = zeros
-            for (int c = threadIdx.x - 64; c < BLOCK_N; c += 128) s_rowvec[c] = 0.f;
+            for (int c = threadIdx.x; c < BLOCK_N; c += 128) s_rowvec[c] = 0.f;
         }
         if (ep.bias != nullptr) {
-            for (int c = threadIdx.x - 64; c < BLOCK_N; c += 128)
+            for (int c = threadIdx.x; c < BLOCK_N; c += 128)
                 s_bias[c] = (col_base + c < p.N) ? __ldg(ep.bias + col_base + c) : 0.f;
         } else if (LINEAR) {
-            for (int c = threadIdx.x - 64; c < BLOCK_N; c += 128) s_bias[c] = 0.f;
+            for (int c = threadIdx.x; c < BLOCK_N; c += 128) s_bias[c] = 0.f;
         }
-        uint4 rcur[4];
-        auto load_res = [&](int c0, uint4(&rv)[4]) {
-#pragma unroll
-            for (int g = 0; g < 4; ++g) {
-                const int cg = col_base + c0 + g * 8;
-                rv[g] = (res != nullptr && cg < p.N) ? __ldg(reinterpret_cast<const uint4*>(res + cg))
-                                                     : make_uint4(0u, 0u, 0u, 0u);
-            }
-        };
-        if (!BULK_RES && !split) load_res(0, rcur);
-        float ln_mean = 0.f, ln_rstd = 0.f;
         if constexpr (LN_CONSUME) {
             if (row_ok) {  // fixed-order fold of the producer's per-tile partials -> mean / rstd of my row of A
                 const float2* sp = reinterpret_cast<const float2*>(ep.row_stats_in) + pix * ep.stats_in_ld;
@@ -290,14 +233,75 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                 ln_rstd = rsqrtf(fmaxf(fmaf(-ln_mean, ln_mean, s2 * inv), 0.f) + ep.ln_eps);
             }
         }
-        float st1 = 0.f, st2 = 0.f;  // producer: my row's statistics over this tile's columns
-        asm volatile("bar.sync 1, 128;" ::: "memory");  // s_bias / s_rowvec visible to the four epilogue warps
+    }
 
-        mbar_wait(tmem_full_bar, 0);
+    // ---- mainloop: each warpgroup multiplies its 64 rows of A by the whole B tile; the previous stage is released once
+    // the MMAs that read it have retired (wait_group 1 keeps one group in flight)
+    {
+        float acc[BLOCK_N / 2];
+#pragma unroll
+        for (int j = 0; j < BLOCK_N / 2; ++j) acc[j] = 0.f;
+        const bool leader = (threadIdx.x & 127) == 0;
+        for (int i = 0; i < nk; ++i) {
+            const int stage = i % STAGES;
+            mbar_wait_quiet(&full_bar[stage], (i / STAGES) & 1);
+            if (i == 0 && threadIdx.x == 0) dbg_mark(p, 2);
+            const uint32_t sa = smem_u32(smem + stage * L::kStageBytes) + wg * (64 * 128);
+            const uint32_t sb = smem_u32(smem + stage * L::kStageBytes) + kABytes;
+            wgmma_fence_regs(acc);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < kBlockK / 16; ++k) {
+                const uint64_t ad = wgmma_desc_sw128(sa + k * 32), bd = wgmma_desc_sw128(sb + k * 32);
+                if constexpr (BLOCK_N == 64) wgmma_m64n64k16(acc, ad, bd, 1u);
+                else if constexpr (BLOCK_N == 128) wgmma_m64n128k16(acc, ad, bd, 1u);
+                else if constexpr (BLOCK_N == 160) wgmma_m64n160k16(acc, ad, bd, 1u);
+                else wgmma_m64n256k16(acc, ad, bd, 1u);
+            }
+            wgmma_commit();
+            wgmma_wait<1>();
+            wgmma_fence_regs(acc);
+            if (i > 0 && leader) mbar_arrive(&empty_bar[(i - 1) % STAGES]);
+        }
+        wgmma_wait<0>();
+        wgmma_fence_regs(acc);
+        // every MMA of the CTA has to retire before the ring is overwritten by the accumulator rows
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+        if (threadIdx.x == 0) dbg_mark(p, 3);
         if (p.pdl_late) pdl_launch_dependents();  // mainloop done: the next kernel's prologue may overlap this epilogue
-        tc_fence_after();
-        if (threadIdx.x == 64) dbg_mark(p, 4);
-        const uint32_t taddr = tmem_base + (static_cast<uint32_t>(lane_group * 32) << 16);
+        // wgmma m64nN accumulator layout: warp w of the warpgroup holds rows 16 w + lane / 4 (+ 8), columns 8 j + 2 (lane % 4)
+        const int wrow = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+#pragma unroll
+        for (int j = 0; j < BLOCK_N / 8; ++j) {
+            const int col = j * 8 + 2 * (lane & 3);
+            *reinterpret_cast<float2*>(smem + wrow * L::kAccRowBytes + col * 4) = make_float2(acc[4 * j], acc[4 * j + 1]);
+            *reinterpret_cast<float2*>(smem + (wrow + 8) * L::kAccRowBytes + col * 4) =
+                make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+        }
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+    }
+    if (wg != 0) return;
+
+    {
+        // ---------------- epilogue (warpgroup 0, thread = tile row) ----------------
+        const float alpha = ep.alpha;
+        const __nv_bfloat16* res = nullptr;
+        if (ep.residual != nullptr && row_ok)
+            res = reinterpret_cast<const __nv_bfloat16*>(ep.residual) + pix * ep.ldr;
+        const bool split = p.splits > 1;
+        uint8_t* acc_row = smem + r * L::kAccRowBytes;
+        uint4 rcur[4];
+        auto load_res = [&](int c0, uint4(&rv)[4]) {
+#pragma unroll
+            for (int g = 0; g < 4; ++g) {
+                const int cg = col_base + c0 + g * 8;
+                rv[g] = (res != nullptr && cg < p.N) ? __ldg(reinterpret_cast<const uint4*>(res + cg))
+                                                     : make_uint4(0u, 0u, 0u, 0u);
+            }
+        };
+        if (!split) load_res(0, rcur);
+        float st1 = 0.f, st2 = 0.f;  // producer: my row's statistics over this tile's columns
+        if (threadIdx.x == 0) dbg_mark(p, 4);
 
         // ---- split-K rendezvous
         const int64_t tile_elems = static_cast<int64_t>(kBlockM) * BLOCK_N;
@@ -307,34 +311,32 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             float* mine = p.ws + (static_cast<int64_t>(blockIdx.z) * n_tiles_total + tile_id) * tile_elems +
                           static_cast<int64_t>(r) * BLOCK_N;
 #pragma unroll 1
-            for (int c0 = 0; c0 < BLOCK_N; c0 += 32) {
-                uint32_t v[32];
-                tmem_ld32(taddr + c0, v);
-                tmem_ld_wait();
-#pragma unroll
-                for (int j = 0; j < 32; j += 4)
-                    __stcg(reinterpret_cast<float4*>(mine + c0 + j),
-                           make_float4(__uint_as_float(v[j]), __uint_as_float(v[j + 1]), __uint_as_float(v[j + 2]),
-                                       __uint_as_float(v[j + 3])));
-            }
+            for (int c0 = 0; c0 < BLOCK_N; c0 += 4)
+                __stcg(reinterpret_cast<float4*>(mine + c0), *reinterpret_cast<const float4*>(acc_row + c0 * 4));
             __threadfence();
-            asm volatile("bar.sync 1, 128;" ::: "memory");
-            if (threadIdx.x == 64) {  // first epilogue thread
+            asm volatile("bar.sync 2, 128;" ::: "memory");
+            if (threadIdx.x == 0) {
                 const unsigned int old = atomicAdd(&p.counters[tile_id], 1u);
-                *tmem_slot = (old == static_cast<unsigned int>(p.splits - 1)) ? 1u : 0u;  // slot is free to reuse now
+                *flag_slot = (old == static_cast<unsigned int>(p.splits - 1)) ? 1u : 0u;
                 if (old == static_cast<unsigned int>(p.splits - 1)) p.counters[tile_id] = 0u;  // re-arm for next launch
             }
-            asm volatile("bar.sync 1, 128;" ::: "memory");
-            const bool last = *reinterpret_cast<volatile uint32_t*>(tmem_slot) != 0u;
-            if (!last) goto epilogue_done;
+            asm volatile("bar.sync 2, 128;" ::: "memory");
+            const bool last = *reinterpret_cast<volatile uint32_t*>(flag_slot) != 0u;
+            if (!last) {
+                if (threadIdx.x == 0) dbg_mark(p, 5);
+                return;
+            }
             __threadfence();
-            if (!BULK_RES) load_res(0, rcur);
+            load_res(0, rcur);
         }
-        // accumulator chunk loader: TMEM (single CTA per tile) or the fixed-order sum of the split partials
+        // accumulator chunk loader: my staged row (single CTA per tile) or the fixed-order sum of the split partials
         auto load_acc = [&](int c0, uint32_t(&v)[32]) {
             if (!split) {
-                tmem_ld32(taddr + c0, v);
-                tmem_ld_wait();
+#pragma unroll
+                for (int j = 0; j < 32; j += 4) {
+                    const uint4 t = *reinterpret_cast<const uint4*>(acc_row + (c0 + j) * 4);
+                    v[j] = t.x; v[j + 1] = t.y; v[j + 2] = t.z; v[j + 3] = t.w;
+                }
             } else {
                 float acc[32];
 #pragma unroll
@@ -356,38 +358,13 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         if constexpr (LINEAR) {
             constexpr int NCH = BLOCK_N / 32;
             __nv_bfloat16* orow = reinterpret_cast<__nv_bfloat16*>(p.out) + pix * p.ldd + col_base;
-            uint32_t v[2][32];
-            const bool res_staged = BULK_RES && ep.residual != nullptr;  // uniform over the CTA
-            if constexpr (BULK_RES) {
-                if (res_staged) {  // the operand ring is idle (every MMA has retired): my residual row -> my staging row
-                    uint64_t* res_bar = reinterpret_cast<uint64_t*>(smem + L::kResBarOffset) + lane_group;
-                    const int valid_cols = min(BLOCK_N, p.N - col_base);
-                    const unsigned rows_ok = __popc(__ballot_sync(0xffffffffu, row_ok && valid_cols > 0));
-                    if (lane == 0) mbar_arrive_expect_tx(res_bar, rows_ok * static_cast<uint32_t>(valid_cols) * 2u);
-                    __syncwarp();
-                    if (row_ok && valid_cols > 0)
-                        bulk_load_g2s(smem_u32(smem + r * kRowStage), res + col_base, static_cast<uint32_t>(valid_cols) * 2u,
-                                      res_bar);
-                    if (!split) tmem_ld32(taddr, v[0]);  // the first accumulator chunk travels meanwhile
-                    mbar_wait(res_bar, 0);
-                } else if (!split) {
-                    tmem_ld32(taddr, v[0]);
-                }
-            } else {
-                if (!split) tmem_ld32(taddr, v[0]);
-            }
 #pragma unroll
             for (int ch = 0; ch < NCH; ++ch) {
                 const int c0 = ch * 32;
-                uint32_t(&vc)[32] = v[ch & 1];
-                if (!split) {
-                    tmem_ld_wait_dep(vc);
-                    if (ch + 1 < NCH) tmem_ld32(taddr + c0 + 32, v[(ch + 1) & 1]);  // next chunk in flight
-                } else {
-                    load_acc(c0, vc);
-                }
+                uint32_t vc[32];
+                load_acc(c0, vc);
                 uint4 rnext[4];
-                if (!BULK_RES && ch + 1 < NCH) load_res(c0 + 32, rnext);
+                if (ch + 1 < NCH) load_res(c0 + 32, rnext);
                 if (row_ok && col_base + c0 < p.N) {
 #pragma unroll
                     for (int g = 0; g < 4; ++g) {
@@ -420,13 +397,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                             f[0] += b0.x; f[1] += b0.y; f[2] += b0.z; f[3] += b0.w;
                             f[4] += b1.x; f[5] += b1.y; f[6] += b1.z; f[7] += b1.w;
                         }
-                        uint4 rv = make_uint4(0u, 0u, 0u, 0u);
-                        if constexpr (BULK_RES) {
-                            if (res_staged && col_base + cl < p.N)
-                                rv = *reinterpret_cast<const uint4*>(smem + r * kRowStage + cl * 2);
-                        } else {
-                            rv = rcur[g];  // zeros when there is no residual
-                        }
+                        const uint4 rv = rcur[g];  // zeros when there is no residual
                         f[0] += bf16lo(rv.x); f[1] += bf16hi(rv.x); f[2] += bf16lo(rv.y); f[3] += bf16hi(rv.y);
                         f[4] += bf16lo(rv.z); f[5] += bf16hi(rv.z); f[6] += bf16lo(rv.w); f[7] += bf16hi(rv.w);
                         const uint4 o = make_uint4(pack_bf16x2(f[0], f[1]), pack_bf16x2(f[2], f[3]),
@@ -443,22 +414,21 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                             }
                         }
                         if constexpr (BULK) {
-                            *reinterpret_cast<uint4*>(smem + r * kRowStage + cl * 2) = o;  // ring is idle: all MMAs retired
+                            // bytes [2 cl, 2 cl + 16) of my row: accumulator columns this thread has already read
+                            *reinterpret_cast<uint4*>(acc_row + cl * 2) = o;
                         } else {
                             if (col_base + cl < p.N) *reinterpret_cast<uint4*>(orow + cl) = o;
                         }
                     }
                 }
-                if constexpr (!BULK_RES) {
 #pragma unroll
-                    for (int g = 0; g < 4; ++g) rcur[g] = rnext[g];
-                }
+                for (int g = 0; g < 4; ++g) rcur[g] = rnext[g];
             }
             if constexpr (BULK) {
                 // each thread ships its own row: generic-proxy writes -> async-proxy read needs the proxy fence only
                 fence_proxy_async_smem();
                 const int valid = min(BLOCK_N, p.N - col_base);
-                if (row_ok && valid > 0) bulk_store_s2g(orow, smem_u32(smem + r * kRowStage), static_cast<uint32_t>(valid) * 2u);
+                if (row_ok && valid > 0) bulk_store_s2g(orow, smem_u32(acc_row), static_cast<uint32_t>(valid) * 2u);
                 bulk_commit();
                 bulk_wait_read0();  // the staging bytes must stay valid until the copy engine has read them
             }
@@ -472,14 +442,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 #pragma unroll 1
                 for (int c0 = 0; c0 < 64; c0 += 32) {
                     uint32_t va[32], vg[32];
-                    if (!split) {  // both halves in flight, one wait
-                        tmem_ld32(taddr + c0, va);
-                        tmem_ld32(taddr + 64 + c0, vg);
-                        tmem_ld_wait();
-                    } else {
-                        load_acc(c0, va);
-                        load_acc(64 + c0, vg);
-                    }
+                    load_acc(c0, va);
+                    load_acc(64 + c0, vg);
                     const int pcol = n_blk * 128 + c0;  // packed column of value; gate at +64
                     const int ocol = n_blk * 64 + c0;
                     if (row_ok && pcol < p.N) {
@@ -586,12 +550,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             }
         }
     }
-
-epilogue_done:
-    if (threadIdx.x == 64) dbg_mark(p, 5);
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, tmem_cols_for(BLOCK_N));
+    if (threadIdx.x == 0) dbg_mark(p, 5);
 }
 
 // ------------------------------------------------------------------------------------------------ host side
@@ -652,44 +611,32 @@ static int ensure_scratch(float** ws, unsigned int** counters, cudaStream_t stre
 }
 
 // ---- tile / pipeline-depth / split-K choice --------------------------------------------------------------------
-// Variants: N tile 64 / 128 / 160 / 256; "shallow" pipelines (<= 112 KB smem, two CTAs per SM so one CTA's epilogue
-// overlaps the other's mainloop — best when the grid covers the chip more than once) or "deep" ones (~190 KB, one
-// CTA per SM with twice the bytes in flight — best when there are fewer CTAs than SMs and each CTA is bound by the
-// latency of its own TMA ring); split-K for the deep UNet levels whose output has only a handful of tiles.
-// The choice is table-driven: csrc/gemm_tuning.inc holds the measured-best variant for every problem the UNet /
-// ControlNet issue at the benchmarked batch sizes (tools/gemm_sweep.py); unseen problems use the rule below,
-// which was read off the same measurements.
+// Variants: N tile 64 / 128 / 160 / 256 with a "shallow" (2-4 stages) or "deep" (4-8 stages, ~190 KB) operand ring. Every
+// variant runs one CTA per SM; the shared-memory footprint is max(ring, 128 x (4 BN + 16) bytes of accumulator staging)
+// plus the epilogue vectors (about 96-200 KB). Deep rings keep more bytes in flight for grids of at most one wave, where
+// each CTA is bound by the latency of its own TMA ring; split-K serves the deep UNet levels whose output has only a
+// handful of tiles. The thresholds below are a rule of thumb in units of the 132 SMs, not tuned by measurement on H100.
 struct GemmCfg {
     int bn, stages, splits;
 };
-struct TuneEntry {
-    int m_tiles, N, kb_total, geglu, bn, stages, splits;
-};
-static const TuneEntry kTuneTable[] = {
-#include "gemm_tuning.inc"
-    {0, 0, 0, 0, 0, 0, 0}};
 
 static int shallow_stages(int bn) { return bn == 64 ? 4 : (bn == 256 ? 2 : 3); }
 static int deep_stages(int bn) { return bn == 64 ? 8 : (bn == 128 ? 6 : (bn == 160 ? 5 : 4)); }
 
 static GemmCfg choose_cfg(int m_tiles, int N, int kb_total, bool geglu) {
-    for (const TuneEntry* e = kTuneTable; e->bn != 0; ++e)
-        if (e->m_tiles == m_tiles && e->N == N && e->kb_total == kb_total && e->geglu == (geglu ? 1 : 0))
-            return {e->bn, e->stages, e->splits};
-    // fallback rule
     auto ctas = [&](int bn) { return static_cast<int64_t>(m_tiles) * ((N + bn - 1) / bn); };
-    if (geglu) return {128, ctas(128) > 160 ? 3 : 6, 1};
-    if (ctas(160) >= 400) return {160, 3, 1};                      // many waves: widest 2-CTA/SM tile
+    if (geglu) return {128, ctas(128) > kNumSms ? 3 : 6, 1};
+    if (ctas(160) >= 3 * kNumSms) return {160, 3, 1};  // many waves: widest 2-CTA/SM tile
     int bn = 64;
-    if (ctas(160) >= 150 && ctas(160) <= 296 && (N % 160 == 0 || N > 640)) bn = 160;
-    else if (ctas(128) >= 150) bn = 128;
+    if (ctas(160) >= kNumSms && ctas(160) <= 2 * kNumSms && (N % 160 == 0 || N > 640)) bn = 160;
+    else if (ctas(128) >= kNumSms) bn = 128;
     int splits = 1;
-    if (ctas(bn) < 100 && kb_total >= 60) {
-        splits = static_cast<int>((160 + ctas(bn) - 1) / ctas(bn));
+    if (ctas(bn) < kNumSms * 2 / 3 && kb_total >= 60) {
+        splits = static_cast<int>((kNumSms + ctas(bn) - 1) / ctas(bn));
         splits = std::min(splits, std::min(6, kb_total / 30));
         splits = std::max(splits, 1);
     }
-    const bool deep = ctas(bn) * splits <= 180;
+    const bool deep = ctas(bn) * splits <= kNumSms;
     return {bn, deep ? deep_stages(bn) : shallow_stages(bn), splits};
 }
 
@@ -697,11 +644,11 @@ template <int BLOCK_N, int STAGES, int EPI, int LNM = 0>
 static int launch_gemm_impl(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, int m_tiles,
                             cudaStream_t stream) {
     using L = GemmSmem<BLOCK_N, STAGES>;
-    constexpr int kSmem = EPI == 3 ? L::kTotalRes : L::kTotal;
+    constexpr int kSmem = L::kTotal;
     IMAGD_SET_MAX_SMEM((gemm_tc_kernel<BLOCK_N, STAGES, EPI, LNM>), kSmem);
     const int n_tiles = (p.N + BLOCK_N - 1) / BLOCK_N;
     dim3 grid(m_tiles, LNM == 3 ? 4 * n_tiles : n_tiles, p.splits);
-    IMAGD_CUDA(launch_pdl(gemm_tc_kernel<BLOCK_N, STAGES, EPI, LNM>, grid, dim3(192), kSmem, stream, tmA, tmB, p));
+    IMAGD_CUDA(launch_pdl(gemm_tc_kernel<BLOCK_N, STAGES, EPI, LNM>, grid, dim3(kGemmThreads), kSmem, stream, tmA, tmB, p));
     return IMAGD_OK;
 }
 
@@ -722,30 +669,19 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const Gem
         set_error("gemm: LayerNorm-folded generic epilogue exists for the GEGLU tile (128) only");
         return IMAGD_ERR_ARG;
     }
-    // Bulk row stores pay off once the grid covers the chip more than twice (measured round 1: +3 % at batch 8,
-    // slightly negative for <= 1-wave grids). IMAGD_GEMM_BULK_STORE = 0 / 1 forces it off / on.
+    // Bulk row stores: for grids that cover the chip more than twice. IMAGD_GEMM_BULK_STORE = 0 / 1 forces them off / on.
     static int bulk_env = -2;
     if (bulk_env == -2) {
         const char* e = getenv("IMAGD_GEMM_BULK_STORE");
         bulk_env = e ? (e[0] == '1' ? 1 : 0) : -1;
     }
     const int64_t ctas = static_cast<int64_t>(m_tiles) * ((p.N + BLOCK_N - 1) / BLOCK_N) * p.splits;
-    const bool bulk = bulk_env >= 0 ? bulk_env == 1 : ctas > 2 * 148;
+    const bool bulk = bulk_env >= 0 ? bulk_env == 1 : ctas > 2 * kNumSms;
     if (!linear) return launch_gemm_impl<BLOCK_N, STAGES, 0>(tmA, tmB, p, m_tiles, stream);
     if (!bulk) return launch_gemm_impl<BLOCK_N, STAGES, 1>(tmA, tmB, p, m_tiles, stream);
-    // The residual also travels by bulk copy through the staging rows (validated on B200 in round 2: all GEMM tests
-    // green with it forced on, batch-8 step 24.49 -> 24.32 ms); IMAGD_GEMM_BULK_RES=0 switches it off.
-    static int bulk_res = -1;
-    if (bulk_res < 0) {
-        const char* e = getenv("IMAGD_GEMM_BULK_RES");
-        bulk_res = (e && e[0] == '0') ? 0 : 1;
-    }
-    const bool res_ok = p.ep.residual != nullptr && p.ep.ldr % 8 == 0;
-    return (bulk_res && res_ok) ? launch_gemm_impl<BLOCK_N, STAGES, 3>(tmA, tmB, p, m_tiles, stream)
-                                : launch_gemm_impl<BLOCK_N, STAGES, 2>(tmA, tmB, p, m_tiles, stream);
+    return launch_gemm_impl<BLOCK_N, STAGES, 2>(tmA, tmB, p, m_tiles, stream);
 }
 
-#include "gemm_persist.inc"
 
 static int g_force_bn = 0, g_force_stages = 0, g_force_splits = 0;  // test hooks (imagd_gemm_debug_force)
 static int g_log_on = 0;
@@ -823,19 +759,7 @@ static int run_gemm_like(const void* A, int64_t lda, int NB, int H, int W, int C
     IMAGD_CHECK_ARG(!ep.row_stats_out || ep.stats_ld >= (N + cfg.bn - 1) / cfg.bn,
                     "gemm: stats_ld=%lld is smaller than the %d N tiles of this launch (imagd_gemm_tile_count_n)",
                     (long long)ep.stats_ld, (N + cfg.bn - 1) / cfg.bn);
-    // opt-in persistent kernel: plain bf16 epilogues of multi-wave problems only
-    bool use_persist = false;
     if (ups_mode) cfg.splits = 1;  // (the split-K scratch is sized for one phase)
-    if (!ups_mode && persist_enabled() && ep.act == IMAGD_ACT_NONE && !ep.out_fp32 && !ep.row_stats_out && !ep.row_stats_in &&
-        (!ep.residual || ep.ldr % 8 == 0)) {
-        const int pbn = persist_block_n(N);
-        if (m_tiles64 * ((N + pbn - 1) / pbn) > 2 * 148) {
-            cfg.bn = pbn;
-            cfg.splits = 1;
-            use_persist = true;
-        }
-    }
-    p.persist_n_tiles = p.persist_total = 0;
     p.ups_n_tiles = ups_mode ? 1 : 0;  // the launcher fills in the real tile count
     p.pdl_late = pdl_mode() == 2 ? 1 : 0;
     p.splits = cfg.splits;
@@ -870,13 +794,6 @@ static int run_gemm_like(const void* A, int64_t lda, int NB, int H, int W, int C
         uint32_t box[2] = {kBlockK, static_cast<uint32_t>(cfg.bn)};
         int rc = make_tmap_bf16(&tmB, Wt, 2, dims, strides, box);
         if (rc != IMAGD_OK) return rc;
-    }
-    if (use_persist) {
-        switch (cfg.bn) {
-            case 160: return launch_persist<160, 3>(tmA, tmB, p, m_tiles, stream);
-            case 128: return launch_persist<128, 4>(tmA, tmB, p, m_tiles, stream);
-            default: return launch_persist<64, 6>(tmA, tmB, p, m_tiles, stream);
-        }
     }
     switch (cfg.bn * 100 + cfg.stages) {
         case 6404: return launch_gemm<64, 4>(tmA, tmB, p, m_tiles, stream);

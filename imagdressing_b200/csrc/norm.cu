@@ -30,14 +30,14 @@ static int gn_max_chunks() {  // IMAGD_GN_MAXCHUNKS, default 64
     if (v == 0) {
         const char* e = getenv("IMAGD_GN_MAXCHUNKS");
         v = e ? atoi(e) : 64;
-        if (v < 1 || v > 148) v = 64;
+        if (v < 1 || v > kNumSms) v = 64;
     }
     return v;
 }
 inline int gn_chunks(int HW, int NB) {
     const int px = gn_pixels_per_chunk();
     int c = (HW + px - 1) / px;
-    const int cap = (148 * 2) / (NB > 0 ? NB : 1);
+    const int cap = (kNumSms * 2) / (NB > 0 ? NB : 1);
     if (c > gn_max_chunks()) c = gn_max_chunks();
     if (c > cap) c = cap;
     return c < 1 ? 1 : c;
@@ -544,9 +544,7 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const __nv_bfloat16* __r
 
 // Which GroupNorm kernel: IMAGD_GN_CLUSTER = 0 the chunked rendezvous kernel always; 1 (default) the cluster kernel in the
 // latency-bound regime it exists for — the whole launch is one wave of clusters and a CTA's tile is at most 32 KB; 2 whenever
-// a slice fits shared memory. Measured on the UNet's shapes at batch 1 (profiles/r02_call29_gn_cluster_bulk.txt, graph-replayed
-// launches): tiles <= 30 KB 8-12 us against 9-21 us for the rendezvous kernel (C = 2560: 8.8 vs 21.3 us); 41 KB tiles mixed
-// (64x64x320 13.5 vs 11.5 us); the 123 KB tile of 64x64x960 29 vs 19 us — hence the cap. Replayed B=1 step 5.54 -> 5.34 ms.
+// a slice fits shared memory. Large tiles stay on the rendezvous kernel, whose shorter CTAs spread them over more SMs.
 static int gn_cluster_mode() {
     static int v = -1;
     if (v < 0) {
@@ -624,7 +622,7 @@ int imagd_groupnorm_stats_bf16(const void* x, int64_t ldx, void* y, int64_t ldy,
                                imagd_stream stream) {
     using namespace imagd;
     IMAGD_CHECK_ARG(x && y && ws, "groupnorm: null pointer");
-    IMAGD_CHECK_ARG(NB > 0 && 2 * NB <= kGnCounters && NB <= 148 * 2 && HW > 0 && C > 0 && C % 8 == 0 && C <= kGnMaxC,
+    IMAGD_CHECK_ARG(NB > 0 && 2 * NB <= kGnCounters && NB <= kNumSms * 2 && HW > 0 && C > 0 && C % 8 == 0 && C <= kGnMaxC,
                     "groupnorm: NB=%d C=%d unsupported", NB, C);
     IMAGD_CHECK_ARG(groups > 0 && groups <= 64 && C % groups == 0, "groupnorm: groups=%d", groups);
     IMAGD_CHECK_ARG(ldx % 8 == 0 && ldy % 8 == 0 && aligned16(x) && aligned16(y), "groupnorm: alignment");

@@ -1,5 +1,5 @@
 // Backward / training-step kernels that are NOT tensor-core work (SURVEY.md section 8 row a13; reference train.py:573-609 gets
-// all of this from torch autograd + DeepSpeed's fused Adam): layout transposes that feed the tcgen05 GEMM its dgrad / wgrad
+// all of this from torch autograd + DeepSpeed's fused Adam): layout transposes that feed the wgmma GEMM its dgrad / wgrad
 // operands, GroupNorm / LayerNorm / activation backward, column reductions (bias and time-embedding gradients), the
 // stride-2 col2im and 2x-upsample adjoints, the MSE loss + its gradient, AdamW. All HBM / L2-bound: 128-bit accesses where
 // the layout allows, fp32 accumulation, fixed-order (bit-reproducible) reductions — no atomics on data.
@@ -760,7 +760,7 @@ extern "C" int imagd_downsum2x_bf16(const void* dy, void* dx, int NB, int H, int
 
 static int colreduce_splits(int rows_per_group, int groups, int C) {
     const int slabs = (C + 63) / 64;
-    int s = (148 * 2) / (slabs * groups > 0 ? slabs * groups : 1);
+    int s = (kNumSms * 2) / (slabs * groups > 0 ? slabs * groups : 1);
     const int by_rows = (rows_per_group + 63) / 64;  // at least 64 rows per split
     if (s > by_rows) s = by_rows;
     if (s > 64) s = 64;
@@ -815,7 +815,7 @@ extern "C" int imagd_layernorm_bwd_bf16(const void* x, int64_t ldx, const void* 
 
 static int gn_bwd_chunks(int HW, int NB) {
     int c = (HW + 15) / 16;
-    const int cap = (148 * 2) / (NB > 0 ? NB : 1);
+    const int cap = (kNumSms * 2) / (NB > 0 ? NB : 1);
     if (c > 64) c = 64;
     if (c > cap) c = cap;
     return c < 1 ? 1 : c;

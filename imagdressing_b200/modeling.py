@@ -1,5 +1,5 @@
 """Host-side mirror of the diffusers-0.24 SD1.5 UNet2DConditionModel / ControlNetModel surface the reference
-drives (SURVEY.md §8b "Host-model surface"), executing on the sm_100a kernels of libimagd_b200.so.
+drives (SURVEY.md §8b "Host-model surface"), executing on the sm_90a kernels of libimagd_b200.so.
 
 The nn.Module tree only *holds* parameters under the diffusers state_dict key names (so the reference's
 checkpoint routing, `.to()`, `.state_dict()`, `set_attn_processor` keep working); arithmetic never goes through
@@ -57,9 +57,8 @@ def skip_default_init():
         nn.Linear.reset_parameters, nn.Conv2d.reset_parameters = saved
 
 
-# LayerNorm folded into the consuming GEMMs of the transformer blocks. Validated on B200 in round 2
-# (profiles/r02_call1_r2prep_validation_ab.txt: eps rel-L2 0.0140 folded vs 0.0144 plain, step 5.80 -> 5.54 ms at B=1,
-# 359 -> 311 launches): on by default, IMAGD_FOLD_LN=0 switches it off; tests flip the module attribute.
+# LayerNorm folded into the consuming GEMMs of the transformer blocks (48 fewer launches per step): on by default,
+# IMAGD_FOLD_LN=0 switches it off; tests flip the module attribute.
 FOLD_LN = os.environ.get("IMAGD_FOLD_LN", "1") == "1"
 
 
@@ -105,7 +104,7 @@ def pack_conv3x3(w: torch.Tensor) -> torch.Tensor:
 
 
 # Upsample2D + conv as four 2x2 phase convs on the low-resolution input (2.25x fewer MACs, no upsampled tensor).
-# Validated on B200 in round 2 (same file); on by default, IMAGD_UPCONV_PHASE=0 switches it off.
+# On by default, IMAGD_UPCONV_PHASE=0 switches it off.
 UPCONV_PHASE = os.environ.get("IMAGD_UPCONV_PHASE", "1") == "1"
 
 

@@ -1,6 +1,6 @@
 """Multi-GPU leg of the path (SURVEY.md §8e): samples are independent, so the global batch is split contiguously
 over ranks (one process per GPU), each rank runs garment pass + 50 steps with zero communication, and the output
-latents meet in ONE all-gather (NCCL over NVLink on the B200 box; gloo in the CPU tests)."""
+latents meet in ONE all-gather (NCCL over NVLink between the GPUs; gloo in the CPU tests)."""
 from __future__ import annotations
 
 from typing import List, Tuple

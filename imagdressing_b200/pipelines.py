@@ -1,6 +1,6 @@
 """The four `IMAGDressing_v1` pipeline classes of the reference (dressing_sd/pipelines/IMAGDressing_v1_pipeline*.py)
 behind their own constructor / `__call__` signatures, driving DenoiseEngine (batched CFG, CUDA-graph replayed
-steps on the sm_100a kernels). The thin modules under dressing_sd/pipelines/ re-export these at the reference's
+steps on the sm_90a kernels). The thin modules under dressing_sd/pipelines/ re-export these at the reference's
 import paths so `inference_IMAGdressing*.py` import them unchanged.
 
 Scope (SURVEY.md §8): the hot path is the garment pass + denoising loop. The edges — CLIP text/vision encoders

@@ -1,6 +1,6 @@
 """CUDA implementations behind the reference's attention-processor plugin API.
 
-`attention_forward` is the one routine all processors share: projection GEMMs (tcgen05), the two-stream attention
+`attention_forward` is the one routine all processors share: projection GEMMs (wgmma), the two-stream attention
 kernel, and the output projection with bias (+ the transformer block's residual when the caller offered it).
 What differs per processor is only which weights are merged (LoRA) and what the second KV stream is:
 

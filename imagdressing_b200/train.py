@@ -1,4 +1,4 @@
-"""Training step of IMAGDressing-v1 on the sm_100a kernels (SURVEY.md section 8 row a13, BASELINE.json configs[4]).
+"""Training step of IMAGDressing-v1 on the sm_90a kernels (SURVEY.md section 8 row a13, BASELINE.json configs[4]).
 
 Mirrors /root/reference/train.py:
   * SDModel                      train.py:244-281  (Resampler -> garment UNet at t = 0 with the cache processors, EVERY batch row
@@ -18,6 +18,7 @@ backward; all arithmetic is in libimagd_b200.so.
 from __future__ import annotations
 
 import math
+import weakref
 from typing import Dict, Iterable, List, Optional
 
 import torch
@@ -377,11 +378,18 @@ class FlatAdamW:
             self._handles.append(torch.distributed.all_reduce(self.grad[lo:hi], async_op=True))
 
     def _make_hook(self, index: int, bucket: int):
+        # weak: a parameter keeps its hooks in the autograd engine's tables, where the garbage collector cannot see a
+        # parameter -> hook -> optimizer -> parameter cycle, so a strong reference would keep every flat buffer alive
+        ref = weakref.ref(self)
+
         def hook(_p):
-            self._ready[bucket].append(index)
-            self._pending[bucket] -= 1
-            if self._pending[bucket] == 0:
-                self._flush_bucket(bucket)
+            opt = ref()
+            if opt is None:
+                return
+            opt._ready[bucket].append(index)
+            opt._pending[bucket] -= 1
+            if opt._pending[bucket] == 0:
+                opt._flush_bucket(bucket)
         return hook
 
     def zero_grad(self):

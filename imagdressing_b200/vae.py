@@ -1,4 +1,4 @@
-"""AutoencoderKL (the SD VAE) on the sm_100a kernels — SURVEY.md §8f row 1, the step either side of the denoising loop:
+"""AutoencoderKL (the SD VAE) on the sm_90a kernels — SURVEY.md §8f row 1, the step either side of the denoising loop:
 
     ref_image_latents = vae.encode(ref_image).latent_dist.mean * 0.18215   dressing_sd/pipelines/IMAGDressing_v1_pipeline.py:454-458
     image             = vae.decode(latents / vae.config.scaling_factor)    :544
@@ -10,9 +10,9 @@ Same surface as diffusers-0.24 `AutoencoderKL` for what the reference touches: `
 to_out.0` and the deprecated `query / key / value / proj_attn` attention names are accepted on load).
 
 Arithmetic (activations bf16 token-major [N, H, W, C], exactly as modeling.py):
-  ResnetBlock2D       GroupNorm+SiLU kernel -> implicit-GEMM conv3x3 (tcgen05) x2, 1x1 shortcut GEMM, residual in the epilogue
+  ResnetBlock2D       GroupNorm+SiLU kernel -> implicit-GEMM conv3x3 (wgmma) x2, 1x1 shortcut GEMM, residual in the epilogue
   Downsample2D        im2col(pad (0,1,0,1)) -> GEMM;     Upsample2D   the four-phase conv on the low-resolution input
-  mid-block attention one head of width 512 does not fit the flash kernel's TMEM budget (O alone would be 512 columns), and
+  mid-block attention one head of width 512 does not fit the flash kernel's register budget (O alone would be 512 columns), and
                       it runs once per image: S = Q K^T (GEMM, fp32 out), row softmax kernel (fp32 statistics, the
                       reference upcasts too), O = P V as a GEMM against V^T — V^T = W_v X^T comes straight out of a GEMM
                       with the operands swapped, and its bias moves into the out-projection (softmax rows sum to one)

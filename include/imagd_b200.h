@@ -1,5 +1,5 @@
 /*
- * imagd_b200.h — C ABI of libimagd_b200.so: the sm_100a kernels behind the IMAGDressing-v1 denoising hot path.
+ * imagd_b200.h — C ABI of libimagd_b200.so: the sm_90a kernels behind the IMAGDressing-v1 denoising hot path.
  *
  * Boundary contract (SURVEY.md §8b, "C-ABI extension"): plain pointers + sizes, no torch types; the caller
  * owns every buffer (kernels never allocate), every launch goes to the caller's stream (so the whole step is
@@ -26,7 +26,7 @@ enum imagd_status {
     IMAGD_OK = 0,
     IMAGD_ERR_ARG = -1,  /* bad shape / alignment / null pointer */
     IMAGD_ERR_CUDA = -2, /* CUDA runtime / driver error */
-    IMAGD_ERR_ARCH = -3  /* device is not sm_100 */
+    IMAGD_ERR_ARCH = -3  /* device is not sm_90 */
 };
 
 enum imagd_act { IMAGD_ACT_NONE = 0, IMAGD_ACT_GEGLU = 1, IMAGD_ACT_SILU = 2, IMAGD_ACT_GELU = 3,
@@ -35,7 +35,7 @@ enum imagd_act { IMAGD_ACT_NONE = 0, IMAGD_ACT_GEGLU = 1, IMAGD_ACT_SILU = 2, IM
 /* ---- library ---- */
 int imagd_version(void);
 const char* imagd_last_error(void);
-/* Returns 100 on a B200 (cc 10.0); IMAGD_ERR_ARCH on anything else; IMAGD_ERR_CUDA with no device. */
+/* Returns 90 on an H100 (cc 9.0); IMAGD_ERR_ARCH on anything else; IMAGD_ERR_CUDA with no device. */
 int imagd_device_check(void);
 
 /* ---- fused GEMM / conv epilogue ----
@@ -66,7 +66,7 @@ typedef struct imagd_epilogue {
     const float* colsum;        /* consumer: [N] fp32 */
 } imagd_epilogue;
 
-/* D[M,N] = A[M,K] * W[N,K]^T (+ epilogue).  tcgen05 tensor cores, TMA-fed, fp32 accumulation in TMEM.
+/* D[M,N] = A[M,K] * W[N,K]^T (+ epilogue).  wgmma tensor cores, TMA-fed, fp32 accumulation.
  * Replaces every nn.Linear / 1x1 conv on the path: attn.to_q/to_k/to_v/to_out, to_k_ref/to_v_ref
  * (adapter/attention_processor.py:568-615,598-601), to_k_ip/to_v_ip (:841-842), Transformer2DModel proj_in/out,
  * FeedForward (diffusers-0.24), Resampler linears (adapter/resampler.py:13-20,45-47,186-188).
@@ -100,7 +100,7 @@ int imagd_gemm_debug_log(int enable, char* out, int out_bytes);
 int imagd_gemm_debug_timeline(void* device_buf);
 
 /* Y[n,y,x,:] = sum_{ky,kx} X[n,y+ky-1,x+kx-1,:] * Wt[:, (ky*3+kx)*Cin : +Cin]^T  (stride 1, zero pad 1) as an
- * implicit GEMM on tcgen05: the 9 shifted activation views are fetched by TMA with out-of-bounds zero fill.
+ * implicit GEMM on wgmma: the 9 shifted activation views are fetched by TMA with out-of-bounds zero fill.
  * Replaces ResnetBlock2D.conv1/conv2 and Upsample2D.conv (diffusers-0.24; SURVEY.md Appendix A.2).
  * Cin % 64 == 0.  X: [NB,H,W,ldx], Y: [NB,H,W,ldy]. */
 int imagd_conv3x3_bf16(const void* X, int64_t ldx, int NB, int H, int W, int Cin, const void* Wt, void* Y,
@@ -124,7 +124,7 @@ typedef struct imagd_kv_stream {
 } imagd_kv_stream;
 
 /* out = s0.out_scale * softmax(q k0^T * sm_scale) v0 + s1.out_scale * softmax(q k1^T * sm_scale) v1
- * — two independent softmaxes sharing one Q tile (FlashAttention-style, S/O accumulators in TMEM).
+ * — two independent softmaxes sharing one Q tile (FlashAttention-style, S/O accumulators in registers).
  * Replaces the two F.scaled_dot_product_attention calls + scale-add of RefSAttnProcessor2_0
  * (adapter/attention_processor.py:589-612), the text+IP pair of LoRAIPAttnProcessor2_0 (:833-856), the single
  * SDPA of CAttnProcessor2_0 / CacheAttnProcessor2_0 (:80, :270), and PerceiverAttention's fp32 softmax
@@ -170,7 +170,7 @@ int imagd_im2col3x3_s2_bf16(const void* x, void* col, int NB, int H, int W, int 
 int imagd_im2col3x3_s2_pad_bf16(const void* x, void* col, int NB, int H, int W, int C, int pad_lo, imagd_stream stream);
 /* P[r, :] = softmax(scale * S[r, :]): fp32 scores [rows, lds] -> bf16 probabilities [rows, ldp]; cols % 4 == 0,
  * cols <= 16384. The softmax of the VAE mid-block attention (one head of width 512: AutoencoderKL, diffusers-0.24
- * Attention with upcast_softmax; reference call sites IMAGDressing_v1_pipeline.py:457,544), between two tcgen05 GEMMs. */
+ * Attention with upcast_softmax; reference call sites IMAGDressing_v1_pipeline.py:457,544), between two GEMMs. */
 int imagd_softmax_rows(const float* s, int64_t lds, void* p, int64_t ldp, int64_t rows, int cols, float scale,
                        imagd_stream stream);
 /* Direct (SIMT) 3x3 conv, pad 1, stride 1 or 2, for the thin ends of the network where a tensor-core tile would
@@ -252,7 +252,7 @@ int imagd_attention_train_fwd_bf16(const void* q, int64_t q_ld, void* out, int64
  * caller initialised them (0). */
 int imagd_attention_bwd_prep(const void* d_out, int64_t do_ld, const void* o0, const void* o1, int64_t ld_s, float w0, float w1,
                              float* dsum, int B, int Lq, int heads, int head_dim, int lq_pad, imagd_stream stream);
-/* Backward of the two-stream attention (recompute-S flash style on tcgen05, deterministic, no atomics):
+/* Backward of the two-stream attention (recompute-S flash style, deterministic, no atomics):
  *   dq [B*Lq, dq_ld]           += over both streams   (NULL: skipped)
  *   dk_s / dv_s                 same layout as the stream's k / v (row stride dkv_s_ld, sample stride = the stream's
  *                               sample_rows or len)      (NULL pair: that stream's key / value gradients are skipped)

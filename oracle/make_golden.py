@@ -1,8 +1,6 @@
-"""Generate tests/golden/processors.safetensors by EXECUTING THE REFERENCE'S OWN CODE (unmodified
-/root/reference/adapter/attention_processor.py and adapter/resampler.py) in fp32 on seeded inputs.
-
-Run in the build container only (the GPU box has no /root/reference):
-    python oracle/make_golden.py
+"""Generate tests/golden/{processors,resamplers}.safetensors by EXECUTING THE REFERENCE'S OWN CODE (unmodified
+adapter/attention_processor.py and adapter/resampler.py of a muzishen/IMAGDressing checkout) in fp32 on seeded inputs:
+    python oracle/make_golden.py <path of the reference checkout>
 The reference file needs two diffusers symbols (attention_processor.py:6-7); oracle/_shim supplies them. The `attn`
 argument is oracle.unet.Attention (the diffusers-0.24 Attention surface the processors touch: to_q/to_k/to_v/
 to_out/heads/spatial_norm/group_norm/norm_cross/residual_connection/rescale_output_factor/prepare_attention_mask).
@@ -19,7 +17,8 @@ from safetensors.torch import save_file
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "oracle", "_shim"))
-sys.path.insert(0, "/root/reference")
+REF = os.path.abspath(sys.argv[1]) if len(sys.argv) > 1 else sys.exit("usage: make_golden.py <reference checkout>")
+sys.path.insert(0, REF)
 
 import importlib.util  # noqa: E402
 
@@ -33,12 +32,12 @@ def _load_reference(name, path):
     return mod
 
 
-ref_ap = _load_reference("reference_attention_processor", "/root/reference/adapter/attention_processor.py")  # the reference's file
-ref_rs = _load_reference("reference_resampler", "/root/reference/adapter/resampler.py")
+ref_ap = _load_reference("reference_attention_processor", os.path.join(REF, "adapter", "attention_processor.py"))  # the reference's file
+ref_rs = _load_reference("reference_resampler", os.path.join(REF, "adapter", "resampler.py"))
 
 from oracle.unet import Attention  # noqa: E402
 
-assert ref_ap.__file__.startswith("/root/reference"), ref_ap.__file__
+assert ref_ap.__file__.startswith(REF), ref_ap.__file__
 
 G = torch.Generator().manual_seed(1234)
 
@@ -76,7 +75,7 @@ def put(prefix, module=None, **tensors):
 
 
 torch.set_grad_enabled(False)
-C, H, B, L, LREF, NAME = 160, 4, 2, 96, 128, "down_blocks.0.attentions.0.transformer_blocks.0.attn1.processor"
+C, H, B, L, LREF, NAME = 80, 2, 2, 32, 48, "down_blocks.0.attentions.0.transformer_blocks.0.attn1.processor"
 
 # ---- RefSAttnProcessor2_0 (hybrid self + garment attention), with and without sa_hidden_states
 attn = Attention(C, None, H)
@@ -93,11 +92,11 @@ y = cache(attn, x)
 assert torch.equal(cache.cache["hidden_states"], x)
 put("cache", out=y)
 
-# ---- CAttnProcessor2_0 (text cross-attention, 77 tokens x 256-d here; 768-d in production)
-attn2 = Attention(C, 256, H)
+# ---- CAttnProcessor2_0 (text cross-attention, 77 tokens x 128-d here; 768-d in production)
+attn2 = Attention(C, 128, H)
 fill_(attn2)
-cproc = ref_ap.CAttnProcessor2_0(NAME.replace("attn1", "attn2"), C, 256)
-t = rnd(B, 77, 256)
+cproc = ref_ap.CAttnProcessor2_0(NAME.replace("attn1", "attn2"), C, 128)
+t = rnd(B, 77, 128)
 put("cattn", attn2, x=x.bfloat16(), t=t.bfloat16(), out=cproc(attn2, x, encoder_hidden_states=t, sa_hidden_states={NAME: g}))
 
 # ---- LoraRefSAttnProcessor2_0 (rank 16 here; reference uses 128)
@@ -112,23 +111,23 @@ rlproc.load_state_dict(lproc.state_dict())
 put("reflora", out=rlproc(attn, x, sa_hidden_states={NAME: g}))
 
 # ---- LoRAIPAttnProcessor2_0 (77 text + 4 IP tokens)
-ipproc = ref_ap.LoRAIPAttnProcessor2_0(C, 256, rank=16, lora_scale=0.2, scale=0.9, num_tokens=4)
+ipproc = ref_ap.LoRAIPAttnProcessor2_0(C, 128, rank=16, lora_scale=0.2, scale=0.9, num_tokens=4)
 fill_(ipproc)
-t81 = rnd(B, 81, 256)
+t81 = rnd(B, 81, 128)
 put("loraip.proc", ipproc)
 put("loraip", t=t81.bfloat16(), out=ipproc(attn2, x, encoder_hidden_states=t81),
     out_noface=ipproc(attn2, x, encoder_hidden_states=t))  # B11: last 4 text tokens routed to the IP stream
 
 # ---- Resampler / ProjPlusModel (small dims; same code path as the 768-d production config)
-rs = ref_rs.Resampler(dim=128, depth=2, dim_head=64, heads=2, num_queries=16, embedding_dim=256, output_dim=128, ff_mult=4)
+rs = ref_rs.Resampler(dim=64, depth=2, dim_head=64, heads=2, num_queries=16, embedding_dim=64, output_dim=64, ff_mult=4)
 fill_(rs)
 with torch.no_grad():
     rs.latents.copy_(q(rs.latents))
-clip = rnd(B, 257, 256)
+clip = rnd(B, 33, 64)
 put("resampler", rs, x=clip.bfloat16(), out=rs(clip))
-pp = ref_rs.ProjPlusModel(cross_attention_dim=128, id_embeddings_dim=64, clip_embeddings_dim=256, num_tokens=4)
+pp = ref_rs.ProjPlusModel(cross_attention_dim=64, id_embeddings_dim=32, clip_embeddings_dim=64, num_tokens=4)
 fill_(pp)
-idemb = rnd(B, 64)
+idemb = rnd(B, 32)
 put("projplus", pp, id=idemb.bfloat16(), clip=clip.bfloat16(), out=pp(idemb, clip, shortcut=False),
     out_shortcut=pp(idemb, clip, shortcut=True, scale=0.5))
 
@@ -138,14 +137,18 @@ sproc = ref_ap.SAttnProcessor2_0(NAME, C)
 put("sattn", out=sproc(attn, x, sa_hidden_states={NAME: rnd(B, LREF, C)}), out_nosa=sproc(attn, x))
 g2 = rnd(B, LREF, C)
 put("sattn", g=g2.bfloat16(), out_g=sproc(attn, x, sa_hidden_states={NAME: g2}))
-rcproc = ref_ap.RefCAttnProcessor2_0(NAME.replace("attn1", "attn2"), C, 256, scale=0.7)
+rcproc = ref_ap.RefCAttnProcessor2_0(NAME.replace("attn1", "attn2"), C, 128, scale=0.7)
 fill_(rcproc)
 NAME2 = NAME.replace("attn1", "attn2")
 put("refc.proc", rcproc)
 put("refc", out=rcproc(attn2, x, encoder_hidden_states=t, sa_hidden_states={NAME2: g2}),
     out_nosa=rcproc(attn2, x, encoder_hidden_states=t))
 
-dst = os.path.join(ROOT, "tests", "golden", "processors.safetensors")
-save_file(out, dst, metadata={"generator": "oracle/make_golden.py", "reference": "/root/reference @ 2e8a2bd",
-                              "torch": torch.__version__})
-print(f"wrote {dst}: {len(out)} tensors, {os.path.getsize(dst) / 1e6:.2f} MB")
+# two files (each well under 1 MB): the attention processors, and the Resampler / ProjPlusModel
+meta = {"generator": "oracle/make_golden.py", "reference": "muzishen/IMAGDressing @ 2e8a2bd", "torch": torch.__version__}
+for fname, keep in (("processors.safetensors", lambda k: not k.startswith(("resampler.", "projplus."))),
+                    ("resamplers.safetensors", lambda k: k.startswith(("resampler.", "projplus.")))):
+    dst = os.path.join(ROOT, "tests", "golden", fname)
+    part = {k: v for k, v in out.items() if keep(k)}
+    save_file(part, dst, metadata=meta)
+    print(f"wrote {dst}: {len(part)} tensors, {os.path.getsize(dst) / 1e6:.2f} MB")

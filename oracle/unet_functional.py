@@ -2,8 +2,7 @@
 — TEST INFRASTRUCTURE ONLY (an anchor for oracle/unet.py, VERDICT r1 "next round" item 1b).
 
 Why it exists: `diffusers` is a third-party dependency of the reference (requirements.txt:12, `diffusers==0.24.0`) that
-is absent from /root/reference, from this container and from the GPU box (probed in round 2:
-profiles/r02_call1_probe_ubench.txt, "diffusers ABSENT"), so oracle/unet.py cannot be pinned against the real classes
+is not installed where the suite runs, so oracle/unet.py cannot be pinned against the real classes
 (PARITY UNPINNED for the UNet / ControlNet arithmetic; DESIGN.md section 4). A transcription error shared by
 oracle/unet.py and the product's modeling.py (same nn.Module tree, same author) would pass every test that compares
 the two. This file removes that shared structure: it is a flat FUNCTION over a plain `state_dict` with the diffusers

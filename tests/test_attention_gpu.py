@@ -1,4 +1,4 @@
-"""GPU parity: two-stream tcgen05 attention (through the C ABI) vs the fp32 oracle.
+"""GPU parity: two-stream attention (through the C ABI) vs the fp32 oracle.
 
 Tolerance rel-L2 <= 1e-2: bf16 Q/K/V, fp32 scores and softmax statistics, P rounded to bf16 before P.V
 (as FlashAttention does), bf16 output.
@@ -96,7 +96,7 @@ def test_perceiver_shape(cuda_device):
 
 
 def test_softmax_extreme_scores(cuda_device):
-    """Rows whose max moves block to block (forces the in-TMEM O rescale) and large logits (no overflow)."""
+    """Rows whose max moves block to block (forces the O rescale) and large logits (no overflow)."""
     from imagdressing_b200 import ops
 
     dev = cuda_device

@@ -1,6 +1,8 @@
-"""CPU: the bench.py output contract, checked on the committed driver-format lines of round 2 (profiles/r02_bench_*.json,
-produced by `python bench.py --gpus N --steps 5 --warmup 3` on B200): every key the driver reads is present and typed, the
-roofline / cpu_baseline / e2e objects are complete, and the derived numbers are self-consistent."""
+"""CPU: the bench.py output contract, checked on a committed result line (tests/golden/bench_line_h100_b1.json, produced by
+`python bench.py --gpus 1 --steps 2 --warmup 1` on one H100 SXM at a 700 W power limit; the line records warmup 3,
+the bench's minimum): every key a consumer of the line
+reads is present and typed, the roofline / cpu_baseline / e2e objects are complete, and the derived numbers are
+self-consistent."""
 import json
 import os
 
@@ -9,9 +11,9 @@ import pytest
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-@pytest.mark.parametrize("name,n", [("r02_bench_b1_final.json", 1), ("r02_bench_n2_default.json", 2)])
+@pytest.mark.parametrize("name,n", [("bench_line_h100_b1.json", 1)])
 def test_bench_line_contract(name, n):
-    d = json.load(open(os.path.join(ROOT, "profiles", name)))
+    d = json.load(open(os.path.join(ROOT, "tests", "golden", name)))
     for k, typ in (("metric", str), ("value", float), ("unit", str), ("n_gpus", int), ("steps", int), ("warmup", int),
                    ("ms_per_step", float), ("higher_is_better", bool), ("scaling", str), ("dtype", str), ("data", str),
                    ("config", dict), ("e2e", dict), ("gpu_launches", int), ("clocks", dict), ("roofline", dict)):

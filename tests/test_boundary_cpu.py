@@ -223,13 +223,13 @@ def test_sattn_and_refc_drop_ins_match_reference_goldens(monkeypatch):
     rel = lambda a, b: float((a.float() - b.float()).norm() / b.float().norm())
     name = "down_blocks.0.attentions.0.transformer_blocks.0.attn1.processor"
     name2 = name.replace("attn1", "attn2")
-    C, H = 160, 4
-    attn, attn2 = load(Attention(C, None, H), "refs"), load(Attention(C, 256, H), "cattn")
+    C, H = 80, 2
+    attn, attn2 = load(Attention(C, None, H), "refs"), load(Attention(C, 128, H), "cattn")
     x, g2, t = gold["refs.x"], gold["sattn.g"], gold["cattn.t"]
     sp = ap.SAttnProcessor2_0(name, C)
     assert rel(sp(attn, x, sa_hidden_states={name: g2}), gold["sattn.out_g"]) < 1e-2
     assert rel(sp(attn, x), gold["sattn.out_nosa"]) < 1e-2
-    rc = load(ap.RefCAttnProcessor2_0(name2, C, 256, scale=0.7), "refc.proc")
+    rc = load(ap.RefCAttnProcessor2_0(name2, C, 128, scale=0.7), "refc.proc")
     assert rel(rc(attn2, x, encoder_hidden_states=t, sa_hidden_states={name2: g2}), gold["refc.out"]) < 1e-2
     assert rel(rc(attn2, x, encoder_hidden_states=t), gold["refc.out_nosa"]) < 1e-2
     assert set(rc.state_dict()) == {"to_k_ref.weight", "to_v_ref.weight"}

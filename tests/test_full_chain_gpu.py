@@ -9,10 +9,11 @@ Oracle = `oracle/pipeline.sample_one` in fp32 ON THE GPU (reference-style batch-
 Calibration, not an assumed tolerance: the SAME oracle is also run with its modules in torch bf16 and torch fp16
 (latents kept fp32 between steps, as the product does) and the kernel path must stay within 2x the torch-bf16 drift
 (floor 3e-2). rel-L2 and cosine of the final latents of all three are printed and written to
-gpurun_out/parity_full_chain.json (copied to profiles/ by hand when judged).
+parity_full_chain.json in $IMAGD_PARITY_OUT (default: the system temporary directory).
 """
 import json
 import os
+import tempfile
 
 import pytest
 import torch
@@ -59,7 +60,7 @@ def cosine(a, b):
 
 
 def record(name, **vals):
-    path = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "gpurun_out")
+    path = os.environ.get("IMAGD_PARITY_OUT", tempfile.gettempdir())
     os.makedirs(path, exist_ok=True)
     f = os.path.join(path, "parity_full_chain.json")
     data = json.load(open(f)) if os.path.exists(f) else {}

@@ -1,4 +1,4 @@
-"""GPU parity: tcgen05 GEMM / implicit-GEMM conv3x3 (through the C ABI) vs the fp32 oracle ops.
+"""GPU parity: wgmma GEMM / implicit-GEMM conv3x3 (through the C ABI) vs the fp32 oracle ops.
 
 Tolerance: bf16 inputs, fp32 accumulation, bf16 output -> rel-L2 <= 1e-2 (SURVEY.md §8c); typical is ~3e-3
 (one bf16 rounding of the output).

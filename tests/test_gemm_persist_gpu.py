@@ -1,15 +1,12 @@
-"""GPU (r2-prep, not yet run on hardware): the persistent GEMM / conv kernel (IMAGD_GEMM_PERSISTENT=1 in the environment
-of the test process — the library reads the switch once) on multi-wave problems with every LINEAR epilogue ingredient."""
-import os
-
+"""GPU: GEMM / conv kernels on multi-wave problems (many times the 132 SMs) with every LINEAR epilogue ingredient — the
+grids where the bulk-store epilogue is selected."""
 import pytest
 import torch
 
 from conftest import rel_l2
 from oracle import ops_ref
 
-pytestmark = [pytest.mark.gpu, pytest.mark.skipif(os.environ.get("IMAGD_GEMM_PERSISTENT") != "1",
-                                                  reason="run with IMAGD_GEMM_PERSISTENT=1")]
+pytestmark = pytest.mark.gpu
 BF = torch.bfloat16
 
 

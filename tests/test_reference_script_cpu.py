@@ -12,9 +12,14 @@ Test infrastructure only: the hub ids the script hard-codes ("stabilityai/sd-vae
 "h94/IP-Adapter") are satisfied by directories of those names under a temporary working directory holding small random-init
 models (a relative path that exists is a local directory for both transformers and our from_pretrained), a toy CLIP BPE
 vocabulary, and a synthetic `{"module": ...}` checkpoint with the `ref_unet.` / `unet.` / `proj.` / `adapter_modules.`
-layout; the kernel wrappers are emulated in torch (tests/emulated_ops.py) because this suite has no GPU. The script itself
-is read from /root/reference at run time and is not copied; the test is skipped where the reference tree does not exist
-(the GPU box).
+layout; the kernel wrappers are emulated in torch (tests/emulated_ops.py) because this suite has no GPU.
+
+The script is reference source and is not copied into this repository. With a reference checkout named by
+$IMAGD_REFERENCE_DIR the script itself runs, and every call it makes across the boundary into this repo (the
+from_pretrained loads, the Resampler / processor / scheduler / pipeline constructors, the dtypes it casts to, the pipeline
+call, the saved grid) is recorded and compared with tests/golden/inference_script_trace.json. Without a checkout the same
+sequence is replayed from that recorded trace (`replay` restates the script's steps, inference_IMAGdressing.py:42-197,
+with every value taken from the trace) and the same assertions run. IMAGD_WRITE_TRACE=1 rewrites the trace from a live run.
 """
 import json
 import os
@@ -27,8 +32,9 @@ import torch
 import emulated_ops
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SCRIPT = "/root/reference/inference_IMAGdressing.py"
-pytestmark = pytest.mark.skipif(not os.path.exists(SCRIPT), reason="reference tree not present")
+REFERENCE_DIR = os.environ.get("IMAGD_REFERENCE_DIR")
+SCRIPT = os.path.join(REFERENCE_DIR, "inference_IMAGdressing.py") if REFERENCE_DIR else None
+TRACE = os.path.join(ROOT, "tests", "golden", "inference_script_trace.json")
 
 UNET_CFG = dict(block_out_channels=[32, 64, 64, 64], cross_attention_dim=64, attention_head_dim=8, norm_num_groups=8)
 VAE_CFG = dict(block_out_channels=[32, 32, 64, 64], norm_num_groups=8)
@@ -120,6 +126,144 @@ def make_checkpoint(tmp, unet):
     return path
 
 
+def _plain(v):
+    """JSON summary of a boundary value: plain values as they are, tensors by shape / dtype, generators by seed."""
+    if v is None or isinstance(v, (bool, int, float, str)):
+        return v
+    if isinstance(v, torch.Tensor):
+        return {"tensor": list(v.shape), "dtype": str(v.dtype)}
+    if isinstance(v, torch.Generator):
+        return {"generator_seed": v.initial_seed()}
+    if isinstance(v, type):
+        return {"class": v.__name__}
+    return {"object": type(v).__name__}
+
+
+def _dtype(m):
+    return str(next(m.parameters()).dtype)
+
+
+def install_recorder(monkeypatch, trace):
+    """Wrap the boundary the script calls into, recording (never altering) what it asks for."""
+    import transformers
+
+    import adapter.attention_processor as ap
+    import adapter.resampler as rs
+    import dressing_sd.pipelines.IMAGDressing_v1_pipeline as dp
+    from imagdressing_b200 import modeling, scheduler, vae
+
+    trace.update(from_pretrained=[], resampler=None, scheduler=None)
+    loaded = []  # (object, index in trace["from_pretrained"])
+
+    for cls in (vae.AutoencoderKL, modeling.UNet2DConditionModel, transformers.CLIPTokenizer, transformers.CLIPTextModel,
+                transformers.CLIPVisionModelWithProjection):
+        def wrap(cls, orig):
+            def from_pretrained(klass, path, *a, **kw):
+                obj = orig.__func__(klass, path, *a, **kw)
+                trace["from_pretrained"].append([cls.__name__, path, kw.get("subfolder")])
+                loaded.append((obj, len(trace["from_pretrained"]) - 1))
+                return obj
+            return classmethod(from_pretrained)
+        monkeypatch.setattr(cls, "from_pretrained", wrap(cls, cls.from_pretrained))
+
+    def ctor(cls, key):
+        orig = cls.__init__
+
+        def init(self, *a, **kw):
+            orig(self, *a, **kw)
+            if key is None:
+                object.__setattr__(self, "_trace_ctor", [list(a), kw])
+            else:
+                trace[key] = [list(a), {k: _plain(v) for k, v in kw.items()}]
+        monkeypatch.setattr(cls, "__init__", init)
+
+    for cls in (ap.RefSAttnProcessor2_0, ap.CAttnProcessor2_0, ap.CacheAttnProcessor2_0):
+        ctor(cls, None)
+    ctor(rs.Resampler, "resampler")
+    ctor(scheduler.DDIMScheduler, "scheduler")
+
+    def role(v):
+        for obj, i in loaded:
+            if v is obj:
+                return {"from_pretrained": i, "dtype": _dtype(v) if isinstance(v, torch.nn.Module) else None}
+        if isinstance(v, rs.Resampler):
+            return {"resampler": True, "dtype": _dtype(v)}
+        return _plain(v)
+
+    orig_init, orig_call = dp.IMAGDressing_v1.__init__, dp.IMAGDressing_v1.__call__
+
+    def pipe_init(self, *a, **kw):
+        trace["pipeline"] = {k: role(v) for k, v in kw.items()}
+        trace["processors"] = {}
+        for part in ("unet", "reference_unet"):
+            procs = kw[part].attn_processors
+            trace["processors"][part] = {n: [type(p).__name__] + p.__dict__.get("_trace_ctor", [[], {}]) for n, p in
+                                         procs.items()}
+        trace["processor_dtype"] = _dtype(torch.nn.ModuleList(kw["unet"].attn_processors.values()))
+        orig_init(self, *a, **kw)
+
+    def pipe_call(self, *a, **kw):
+        trace["call"] = {k: _plain(v) for k, v in kw.items()}
+        return orig_call(self, *a, **kw)
+
+    monkeypatch.setattr(dp.IMAGDressing_v1, "__init__", pipe_init)
+    monkeypatch.setattr(dp.IMAGDressing_v1, "__call__", pipe_call)
+
+
+def replay(trace, ckpt, cloth, out_dir):
+    """inference_IMAGdressing.py:42-197 restated, every value taken from the recorded trace."""
+    import transformers
+    from PIL import Image
+    from torchvision import transforms
+
+    import adapter.attention_processor as ap
+    from adapter.resampler import Resampler
+    from dressing_sd.pipelines.IMAGDressing_v1_pipeline import IMAGDressing_v1
+    from imagdressing_b200 import checkpoint, modeling, scheduler, vae
+
+    classes = {"AutoencoderKL": vae.AutoencoderKL, "UNet2DConditionModel": modeling.UNet2DConditionModel,
+               "CLIPTokenizer": transformers.CLIPTokenizer, "CLIPTextModel": transformers.CLIPTextModel,
+               "CLIPVisionModelWithProjection": transformers.CLIPVisionModelWithProjection}
+    dt = lambda s: getattr(torch, s.split(".")[-1])
+    loaded = [classes[c].from_pretrained(p, **({"subfolder": sub} if sub else {})) for c, p, sub in trace["from_pretrained"]]
+    pipe_kw = {}
+    for k, r in trace["pipeline"].items():
+        if "from_pretrained" in r:
+            obj = loaded[r["from_pretrained"]]
+            pipe_kw[k] = obj.to(dtype=dt(r["dtype"])) if r["dtype"] else obj
+        elif "resampler" in r:
+            a, kw = trace["resampler"]
+            pipe_kw[k] = Resampler(*a, **kw).to(dtype=dt(r["dtype"]))
+        elif r.get("object") == "DDIMScheduler":
+            a, kw = trace["scheduler"]
+            pipe_kw[k] = scheduler.DDIMScheduler(*a, **kw)
+        elif "class" in r:
+            pipe_kw[k] = r["class"]  # classes handed over unused (safety checker / feature extractor)
+    for part in ("unet", "reference_unet"):
+        pipe_kw[part].set_attn_processor({n: getattr(ap, c)(*a, **kw) for n, (c, a, kw) in trace["processors"][part].items()})
+    checkpoint.processor_list(pipe_kw["unet"]).to(dtype=dt(trace["processor_dtype"]))
+    checkpoint.load_module_checkpoint(ckpt, reference_unet=pipe_kw["reference_unet"], image_proj=pipe_kw["ImgProj"],
+                                      unet=pipe_kw["unet"])
+    pipe = IMAGDressing_v1(**pipe_kw)
+
+    call = dict(trace["call"])
+    w, h = call["width"], call["height"]
+    garment = Image.open(cloth).convert("RGB")
+    call["ref_image"] = transforms.Compose([transforms.Resize([h, w]), transforms.ToTensor(),
+                                            transforms.Normalize([0.5], [0.5])])(garment).unsqueeze(0)
+    call["ref_clip_image"] = transformers.CLIPImageProcessor()(images=garment, return_tensors="pt").pixel_values
+    call["generator"] = torch.Generator().manual_seed(call["generator"]["generator_seed"])
+    for k in ("ref_image", "ref_clip_image"):
+        assert list(call[k].shape) == trace["call"][k]["tensor"], k
+    out = pipe(**call).images
+    tiles = [garment.resize((w, h), Image.BICUBIC), out[0]]
+    grid = Image.new("RGB", size=(len(tiles) * w, h))
+    for i, t in enumerate(tiles):
+        grid.paste(t, box=(i * w, 0))
+    os.makedirs(out_dir, exist_ok=True)
+    grid.save(os.path.join(out_dir, os.path.basename(cloth)))
+
+
 def test_unmodified_inference_script_runs_end_to_end(tmp_path, monkeypatch):
     import numpy as np
     from PIL import Image
@@ -154,11 +298,21 @@ def test_unmodified_inference_script_runs_end_to_end(tmp_path, monkeypatch):
         return real_run(self, **kw)
 
     monkeypatch.setattr(pl._DressingPipelineBase, "_run", spy)
-    try:
-        runpy.run_path(SCRIPT, run_name="__main__")
-    finally:
-        for m in [m for m in sys.modules if m == "diffusers" or m.startswith("diffusers.")]:
-            sys.modules.pop(m, None)
+    stored = json.load(open(TRACE)) if os.path.exists(TRACE) else None
+    if SCRIPT is not None:  # the reference's own script, its boundary calls checked against the stored trace
+        trace = {}
+        install_recorder(monkeypatch, trace)
+        try:
+            runpy.run_path(SCRIPT, run_name="__main__")
+        finally:
+            for m in [m for m in sys.modules if m == "diffusers" or m.startswith("diffusers.")]:
+                sys.modules.pop(m, None)
+        trace = json.loads(json.dumps(trace))  # tuples -> lists, as stored
+        if os.environ.get("IMAGD_WRITE_TRACE") == "1":
+            json.dump(trace, open(TRACE, "w"), indent=1, sort_keys=True)
+        assert trace == stored
+    else:  # no reference checkout: the recorded script replayed through the same boundary
+        replay(stored, ckpt, cloth, os.path.join(tmp, "out"))
     out = os.path.join(tmp, "out", "cloth.png")
     assert os.path.exists(out)
     grid = Image.open(out)

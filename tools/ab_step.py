@@ -1,7 +1,7 @@
 """A/B the replayed denoising step under several environment settings in ONE GPU call: each configuration runs
 tools/step_timing.py in its own process (the library reads its knobs once) for every batch size; prints one table.
 
-    python tools/ab_step.py "base:" "fold:IMAGD_FOLD_LN=1" "bulkres:IMAGD_GEMM_BULK_RES=1" [--batches 1,8]
+    python tools/ab_step.py "base:" "fold:IMAGD_FOLD_LN=1" "bulk:IMAGD_GEMM_BULK_STORE=1" [--batches 1,8]
 """
 import os
 import re

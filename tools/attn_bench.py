@@ -1,6 +1,6 @@
 """Times the level-0 hybrid attention (head_dim 40, L = 4096, CFG pair per sample: B conditional samples with the garment
 stream + B unconditional) in isolation: CUDA events on the launching stream, L2 flushed between launches.
-    B=1 python tools/attn_bench.py        IMAGD_ATTN_PTMEM=0 B=8 python tools/attn_bench.py
+    B=1 python tools/attn_bench.py        B=8 python tools/attn_bench.py
 Prints algorithmic TFLOP/s (4 L (L + L_ref) C per conditional sample, 4 L L C per unconditional) and the fraction of the
 measured burst bf16 peak (MEASURED_PEAKS.json)."""
 import json
@@ -13,7 +13,7 @@ import torch
 from imagdressing_b200 import ops
 
 dev = torch.device("cuda:0")
-peak = 1691.8
+peak = 989.0  # H100 SXM data sheet, dense bf16 (MEASURED_PEAKS.json overrides)
 try:
     peak = json.load(open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json")))["bf16_tflops"]
 except Exception:
@@ -44,5 +44,5 @@ for B in [int(b) for b in os.environ.get("B", "1,8").split(",")]:
         ms = sorted(ts)[len(ts) // 2]
         fl = 4.0 * L * L * C * (NB + B)
         tf = fl / (ms * 1e-3) / 1e12
-        print(f"PTMEM={os.environ.get('IMAGD_ATTN_PTMEM', '1')} B={B} L={L} hd={C // heads}: {ms * 1e3:.1f} us  {tf:.1f} TFLOP/s  "
+        print(f"B={B} L={L} hd={C // heads}: {ms * 1e3:.1f} us  {tf:.1f} TFLOP/s  "
               f"{tf / peak:.3f} of measured burst peak", flush=True)

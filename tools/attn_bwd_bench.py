@@ -1,6 +1,6 @@
 """Times the two-stream attention backward at the level-0 shape of the training step (micro-batch 4, 5120 tokens, 8 x 40):
 CUDA events on the launching stream, L2 flushed between launches; dQ kernel + dK/dV kernel per stream + the D prep.
-    IMAGD_BWD_DKV2=1 IMAGD_BWD_PACK=2 python tools/attn_bwd_bench.py"""
+    python tools/attn_bwd_bench.py"""
 import os
 import sys
 
@@ -40,5 +40,5 @@ for (B, L, C, heads) in ((4, 5120, 320, 8), (4, 1280, 640, 8), (4, 320, 1280, 8)
             e1.record()
             torch.cuda.synchronize()
             ts.append(e0.elapsed_time(e1))
-        print(f"DKV2={os.environ.get('IMAGD_BWD_DKV2', '0')} PACK={os.environ.get('IMAGD_BWD_PACK', '0')} B={B} L={L} hd={C // heads} "
+        print(f"B={B} L={L} hd={C // heads} "
               f"{name:16s}: {sorted(ts)[3] * 1e3:8.1f} us", flush=True)

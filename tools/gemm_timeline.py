@@ -1,4 +1,4 @@
-"""Per-CTA timeline of the tcgen05 GEMM (imagd_gemm_debug_timeline): where a CTA's lifetime goes for the short-K
+"""Per-CTA timeline of the wgmma GEMM (imagd_gemm_debug_timeline): where a CTA's lifetime goes for the short-K
 transformer GEMMs. Prints the median clocks of each phase over all CTAs + the event-timed kernel duration."""
 import os
 import sys
