@@ -173,6 +173,53 @@ __device__ __forceinline__ void wgmma_m64n256k16(float (&d)[128], uint64_t a_des
         : "l"(a_desc), "l"(b_desc), "r"(scale_d));
 }
 
+// Descriptor for an MN-major ("transposed") B operand in the same 128-byte swizzle: rows of 64 N-elements (128 B) per K
+// index, 8-row / 1024-byte atoms along K (stride byte offset), and the next 64 N-elements `lbo_bytes` further on (leading
+// byte offset). A K step of 16 elements is +2048 bytes on the start address. This is how TMA lays out a [K rows][N cols]
+// tile that is loaded in boxes 64 columns wide, box after box.
+__device__ __forceinline__ uint64_t wgmma_desc_sw128_mn(uint32_t saddr, uint32_t lbo_bytes) {
+    uint64_t d = 0;
+    d |= static_cast<uint64_t>((saddr >> 4) & 0x3FFF);
+    d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
+    d |= static_cast<uint64_t>(1024 >> 4) << 32;
+    d |= static_cast<uint64_t>(1) << 62;
+    return d;
+}
+template <int R>
+__device__ __forceinline__ void wgmma_fence_regs(uint32_t (&d)[R][4]) {
+#pragma unroll
+    for (int i = 0; i < R; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) asm volatile("" : "+r"(d[i][j])::"memory");
+}
+
+// D[64 x N] (+)= A[64 x 16] * B[16 x N]: A from registers (the m16n8k16 A fragment of each warp's 16 rows, which is also
+// how a 64 x 16 slice of a wgmma accumulator is distributed once packed to bf16 pairs), B MN-major in shared memory.
+// The A registers are read asynchronously: they must stay unmodified (wgmma_fence_regs) until the group is waited for.
+__device__ __forceinline__ void wgmma_m64n40k16_rs(float (&d)[20], const uint32_t (&a)[4], uint64_t b_desc, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %25, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n40k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19}, {%20, %21, %22, %23}, %24, p, 1, 1, 1;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(scale_d));
+}
+__device__ __forceinline__ void wgmma_m64n80k16_rs(float (&d)[40], const uint32_t (&a)[4], uint64_t b_desc, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %45, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n80k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39}, {%40, %41, %42, %43}, %44, p, 1, 1, 1;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(scale_d));
+}
+
+// Move registers between warpgroups: every warp of the warpgroup executes it; the block starts with the launch-bound
+// allocation (65536 / threads, per SM sub-partition) and the sum over its warpgroups must stay within the register file.
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+
 // ---------------------------------------------------------------- warp-level MMA (attention kernels)
 // D[16 x 8] += A[16 x 16] * B[16 x 8], bf16 inputs, fp32 accumulators. Fragments (g = lane / 4, t = lane % 4):
 //   A: a0 (row g, k 2t..2t+1), a1 (row g+8, k 2t..), a2 (row g, k 2t+8..), a3 (row g+8, k 2t+8..)
