@@ -8,6 +8,8 @@ SURVEY.md §8f row 1) the VAE, all executing on the sm_90a kernels.
 Never shadow a real diffusers install with this package by accident: it is not on the path unless you add it.
 """
 from imagdressing_b200.modeling import ControlNetModel, UNet2DConditionModel  # noqa: F401
+from imagdressing_b200.samplers import (DPMSolverMultistepScheduler, EulerAncestralDiscreteScheduler,  # noqa: F401
+                                        EulerDiscreteScheduler)
 from imagdressing_b200.scheduler import DDIMScheduler  # noqa: F401
 from imagdressing_b200.vae import AutoencoderKL  # noqa: F401
 

@@ -1,11 +1,19 @@
-"""Scheduler names the reference pipelines use in type annotations; only DDIM is implemented (the scripts use DDIM)."""
+"""Scheduler names the reference pipelines use in type annotations. DDIM, DPM-Solver++ and Euler / Euler-ancestral are
+implemented; PNDM and LMS are not."""
+from imagdressing_b200.samplers import (DPMSolverMultistepScheduler, EulerAncestralDiscreteScheduler,  # noqa: F401
+                                        EulerDiscreteScheduler)
 from imagdressing_b200.scheduler import DDIMScheduler  # noqa: F401
 
 
 class _NotBuilt:
     def __init__(self, *a, **k):
-        raise NotImplementedError("only DDIMScheduler is on the IMAGDressing inference path")
+        raise NotImplementedError(f"{type(self).__name__} is not built; available: DDIMScheduler, "
+                                  "DPMSolverMultistepScheduler, EulerDiscreteScheduler, EulerAncestralDiscreteScheduler")
 
 
-DPMSolverMultistepScheduler = EulerAncestralDiscreteScheduler = EulerDiscreteScheduler = _NotBuilt
-LMSDiscreteScheduler = PNDMScheduler = _NotBuilt
+class LMSDiscreteScheduler(_NotBuilt):
+    pass
+
+
+class PNDMScheduler(_NotBuilt):
+    pass

@@ -477,6 +477,78 @@ __global__ void cfg_ddim_step_kernel(const float* __restrict__ eps_c, const floa
     }
 }
 
+// Generic multistep sampler update (DPM-Solver++ 1S/2M, Euler, Euler-ancestral): every one is linear in x, eps, one
+// history tensor and one noise tensor, so the scheduler reduces to a per-step row {dx, de, cx, ce, ch, cz}.
+__global__ void cfg_sampler_step_kernel(const float* __restrict__ eps_c, const float* __restrict__ eps_u, float g,
+                                        float* __restrict__ lat, float* __restrict__ hist,
+                                        const float* __restrict__ step_noise, const float* __restrict__ coef,
+                                        int32_t* __restrict__ step_ptr, const float* __restrict__ mask,
+                                        const float* __restrict__ img, const float* __restrict__ noise,
+                                        const float* __restrict__ blend_coef, int NB, int C, int HW) {
+    pdl_launch_dependents();
+    pdl_wait();
+    unsigned int* done_counter = reinterpret_cast<unsigned int*>(step_ptr + 1);
+    const int step = *step_ptr;
+    const float* row = coef + step * 6;
+    const float dx = row[0], de = row[1], cx = row[2], ce = row[3], ch = row[4], cz = row[5];
+    float bn_a = 1.f, bn_b = 0.f;
+    if (mask) {
+        bn_a = blend_coef[step * 2 + 0];
+        bn_b = blend_coef[step * 2 + 1];
+    }
+    const int64_t total = static_cast<int64_t>(NB) * C * HW;
+    // a zero coefficient skips its operand entirely: an unwritten history (first step) or noise slot may hold NaN
+    const float* z = (step_noise && cz != 0.f) ? step_noise + static_cast<int64_t>(step) * total : nullptr;
+    for (int64_t idx = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; idx < total;
+         idx += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+        const float u = eps_u ? eps_u[idx] : 0.f;
+        const float c = eps_c[idx];
+        const float eps = eps_u ? u + g * (c - u) : c;
+        const float xt = lat[idx];
+        float xn = cx * xt + ce * eps;
+        if (hist) {
+            if (ch != 0.f) xn += ch * hist[idx];
+            hist[idx] = dx * xt + de * eps;  // this step's data prediction, read back by the next step
+        }
+        if (z) xn += cz * z[idx];
+        if (mask) {
+            const int64_t n = idx / (static_cast<int64_t>(C) * HW);
+            const float m = mask[n * HW + idx % HW];
+            const float proper = bn_a * img[idx] + bn_b * noise[idx];
+            xn = (1.f - m) * proper + m * xn;
+        }
+        lat[idx] = xn;
+    }
+    __threadfence();
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        const unsigned int prev = atomicAdd(done_counter, 1u);
+        if (prev == gridDim.x - 1) {
+            *done_counter = 0u;
+            *step_ptr = step + 1;
+        }
+    }
+}
+
+// nchw_f32_to_nhwc_bf16 with the model-input scaling of the sigma-space samplers: v * scale[*step_ptr]
+__global__ void nchw_f32_to_nhwc_bf16_scaled_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ y, int NB,
+                                                    int C, int H, int W, int Cpad, int repeat,
+                                                    const float* __restrict__ scale, const int32_t* __restrict__ step_ptr) {
+    pdl_launch_dependents();
+    pdl_wait();
+    const float s = scale[step_ptr ? *step_ptr : 0];
+    const int64_t total = static_cast<int64_t>(NB) * repeat * H * W * Cpad;
+    for (int64_t idx = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; idx < total;
+         idx += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+        const int c = static_cast<int>(idx % Cpad);
+        const int64_t pix = idx / Cpad;
+        const int64_t hw = pix % (static_cast<int64_t>(H) * W);
+        const int64_t n = (pix / (static_cast<int64_t>(H) * W)) % NB;
+        const float v = c < C ? x[(n * C + c) * H * W + hw] * s : 0.f;
+        y[idx] = __float2bfloat16(v);
+    }
+}
+
 static inline int grid_for(int64_t total, int threads) {
     int64_t g = (total + threads - 1) / threads;
     if (g > kNumSms * 16) g = kNumSms * 16;
@@ -646,6 +718,33 @@ int imagd_cfg_ddim_step(const float* eps_cond, const float* eps_uncond, float gu
     if (grid > kNumSms) grid = kNumSms;
     IMAGD_CUDA(launch_pdl(cfg_ddim_step_kernel, dim3(grid), dim3(256), 0, static_cast<cudaStream_t>(stream), 
         eps_cond, eps_uncond, guidance, latents, coef, step_ptr, mask, image_latents, noise, blend_coef, NB, C, HW));
+    return IMAGD_OK;
+}
+
+int imagd_cfg_sampler_step(const float* eps_cond, const float* eps_uncond, float guidance, float* latents,
+                           float* history, const float* step_noise, const float* coef, int32_t* step_ptr,
+                           const float* mask, const float* image_latents, const float* noise, const float* blend_coef,
+                           int NB, int C, int HW, imagd_stream stream) {
+    using namespace imagd;
+    IMAGD_CHECK_ARG(eps_cond && latents && coef && step_ptr && NB > 0 && C > 0 && HW > 0, "cfg_sampler_step: bad args");
+    IMAGD_CHECK_ARG(!mask || (image_latents && noise && blend_coef), "cfg_sampler_step: inpaint blend needs all operands");
+    const int64_t total = static_cast<int64_t>(NB) * C * HW;
+    int grid = grid_for(total, 256);
+    if (grid > kNumSms) grid = kNumSms;
+    IMAGD_CUDA(launch_pdl(cfg_sampler_step_kernel, dim3(grid), dim3(256), 0, static_cast<cudaStream_t>(stream),
+        eps_cond, eps_uncond, guidance, latents, history, step_noise, coef, step_ptr, mask, image_latents, noise,
+        blend_coef, NB, C, HW));
+    return IMAGD_OK;
+}
+
+int imagd_nchw_f32_to_nhwc_bf16_scaled(const float* x, void* y, int NB, int C, int H, int W, int Cpad, int repeat,
+                                       const float* scale_table, const int32_t* step_ptr, imagd_stream stream) {
+    using namespace imagd;
+    IMAGD_CHECK_ARG(x && y && scale_table && NB > 0 && C > 0 && Cpad >= C && repeat >= 1, "nchw_to_nhwc_scaled: bad args");
+    const int64_t total = static_cast<int64_t>(NB) * repeat * H * W * Cpad;
+    IMAGD_CUDA(launch_pdl(nchw_f32_to_nhwc_bf16_scaled_kernel, dim3(grid_for(total, 256)), dim3(256), 0,
+        static_cast<cudaStream_t>(stream), x, reinterpret_cast<__nv_bfloat16*>(y), NB, C, H, W, Cpad, repeat,
+        scale_table, step_ptr));
     return IMAGD_OK;
 }
 

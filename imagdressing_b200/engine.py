@@ -8,7 +8,8 @@ IMAGDressing_v1_pipeline_ipa_controlnet.py:595-736, IMAGDressing_v1_pipeline_con
 Differences that do not change per-sample results (SURVEY.md Appendix B): the two batch-1 UNet calls run as one
 CFG batch [cond.., uncond..] whose first n samples carry the garment stream (B1/B4); the garment pass runs at
 batch n on the garment tokens only (B2); only the 16 attn1 taps are kept (B3); one captured CUDA graph is
-replayed for all steps — the step index lives in device memory and the fused CFG+DDIM kernel advances it.
+replayed for all steps — the step index lives in device memory and the fused CFG+DDIM kernel (or, for the
+multistep samplers of samplers.py, the generic CFG+sampler-step kernel) advances it.
 """
 from __future__ import annotations
 
@@ -104,11 +105,17 @@ class DenoiseEngine:
         if use_control and self.controlnet is not None and st.get("control_cond") is not None:
             down, mid = self.controlnet(lat, None, st["control_text"], st["control_cond"],
                                         conditioning_scale=st["control_scale"], return_dict=False,
-                                        timestep_table=table, sample_repeat=2)
+                                        timestep_table=table, sample_repeat=2, input_scale=st.get("scale"))
         eps = self.unet.forward_tokens(lat, None, st["text"], st["kwargs"], down, mid, timestep_table=table,
-                                       out=st["eps"], sample_repeat=2)
-        ops.cfg_ddim_step(eps[:n], eps[n:], st["guidance"], lat, st["coef"], st["step_ptr"], mask=st.get("mask"),
-                          image_latents=st.get("image_latents"), noise=st.get("noise"), blend_coef=st.get("blend"))
+                                       out=st["eps"], sample_repeat=2, input_scale=st.get("scale"))
+        if st["ddim"]:
+            ops.cfg_ddim_step(eps[:n], eps[n:], st["guidance"], lat, st["coef"], st["step_ptr"], mask=st.get("mask"),
+                              image_latents=st.get("image_latents"), noise=st.get("noise"), blend_coef=st.get("blend"))
+        else:
+            ops.cfg_sampler_step(eps[:n], eps[n:], st["guidance"], lat, st["coef"], st["step_ptr"],
+                                 history=st.get("history"), step_noise=st.get("step_noise"), mask=st.get("mask"),
+                                 image_latents=st.get("image_latents"), noise=st.get("noise"),
+                                 blend_coef=st.get("blend"))
 
     def _refresh(self, st) -> bool:
         """Per-image refresh of the step-invariant projections without running a step. Returns False when a
@@ -145,18 +152,30 @@ class DenoiseEngine:
                control_prompt_embeds: Optional[torch.Tensor] = None, control_negative_embeds: Optional[torch.Tensor] = None,
                control_scale: float = 1.0, mask: Optional[torch.Tensor] = None,
                image_latents: Optional[torch.Tensor] = None, noise: Optional[torch.Tensor] = None,
-               callback=None, control_keep: Optional[List[float]] = None) -> torch.Tensor:
-        """latents [n,4,h,w] (scaled by init_noise_sigma = 1); embeds [n,T,768] (or [1,T,768], broadcast).
-        control_keep: per-step 0/1 ControlNet guidance window (`controlnet_keep` of
+               callback=None, control_keep: Optional[List[float]] = None, scheduler=None,
+               step_noise: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """latents [n,4,h,w] (already scaled by the scheduler's init_noise_sigma); embeds [n,T,768] (or [1,T,768],
+        broadcast). control_keep: per-step 0/1 ControlNet guidance window (`controlnet_keep` of
         IMAGDressing_v1_pipeline_ipa_controlnet.py:584-590,643-649); steps with 0 run the UNet without residuals (what
-        a zero conditioning scale computes) from a second captured graph. Returns the final latents as a new fp32 tensor."""
+        a zero conditioning scale computes) from a second captured graph. scheduler: the sampler to run (default: the
+        one given at construction); DDIMScheduler runs the fused CFG+DDIM kernel, the multistep samplers
+        (samplers.py) the generic sampler-step kernel. step_noise: [S,n,4,h,w], one noise draw per step, for samplers
+        that add noise (Euler-ancestral). Returns the final latents as a new fp32 tensor."""
         dev = latents.device
         n = latents.shape[0]
-        sch = self.scheduler
+        sch = scheduler if scheduler is not None else self.scheduler
         if timesteps is None:
             sch.set_timesteps(num_inference_steps, device=dev)
             timesteps = sch.timesteps
-        t_table, coef, blend = sch.step_tables(dev, timesteps)
+        ddim = isinstance(sch, DDIMScheduler)
+        if ddim:
+            t_table, coef, blend = sch.step_tables(dev, timesteps)
+            tables = None
+        else:
+            tables = sch.sampler_tables(dev, timesteps)
+            t_table, coef, blend = tables.t, tables.coef, tables.blend
+            if tables.noise and (step_noise is None or tuple(step_noise.shape) != (t_table.numel(), *latents.shape)):
+                raise ValueError(f"{type(sch).__name__} needs step_noise of shape [steps, *latents.shape]")
         S = t_table.numel()
 
         def bn(t):
@@ -164,7 +183,7 @@ class DenoiseEngine:
 
         has_control = self.controlnet is not None and control_cond is not None
         key = (n, tuple(latents.shape[1:]), prompt_embeds.shape[1], has_control, mask is not None,
-               float(guidance_scale), float(control_scale), bool(sa_hidden_states), id(t_table),
+               float(guidance_scale), float(control_scale), bool(sa_hidden_states), id(t_table), id(coef),
                tuple(control_cond.shape) if has_control else None, self._frozen_signature())
         keep = [1.0] * S if control_keep is None or not has_control else [float(k) for k in control_keep]
         if len(keep) != S or any(k not in (0.0, 1.0) for k in keep):
@@ -176,7 +195,14 @@ class DenoiseEngine:
                       text=torch.empty(2 * n, prompt_embeds.shape[1], prompt_embeds.shape[2], device=dev, dtype=torch.bfloat16),
                       guidance=float(guidance_scale), coef=coef, t_table=t_table,
                       step_ptr=torch.zeros(2, dtype=torch.int32, device=dev),
-                      eps=torch.empty(2 * n, *latents.shape[1:], **f32), kwargs={}, graph=None, graph_nc=None)
+                      eps=torch.empty(2 * n, *latents.shape[1:], **f32), kwargs={}, graph=None, graph_nc=None,
+                      ddim=ddim)
+            if tables is not None:  # (the key holds id(coef) of these live tables: no other sampler replays this graph)
+                st.update(scale=tables.scale)
+                if tables.history:
+                    st.update(history=torch.empty(n, *latents.shape[1:], **f32))
+                if tables.noise:
+                    st.update(step_noise=torch.empty(S, n, *latents.shape[1:], **f32))
             if has_control:
                 cp = control_prompt_embeds if control_prompt_embeds is not None else prompt_embeds
                 st.update(control_cond=torch.empty(control_cond.shape, **f32), control_scale=float(control_scale),
@@ -202,6 +228,8 @@ class DenoiseEngine:
             st["mask"].copy_(mask)
             st["image_latents"].copy_(image_latents)
             st["noise"].copy_(noise)
+        if "step_noise" in st:
+            st["step_noise"].copy_(step_noise)
         st["step_ptr"].zero_()
         if sa_hidden_states:
             # the garment taps are rewritten in place by the captured garment pass: tensor identity/version say

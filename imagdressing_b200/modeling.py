@@ -655,8 +655,11 @@ class _ModelBase(nn.Module):
         return encoder_hidden_states.to(BF16).contiguous()
 
 
-def _to_tokens(sample: torch.Tensor, repeat: int = 1) -> torch.Tensor:
-    """[N, C, H, W] (any float dtype) -> bf16 [N*repeat, H, W, C] via the layout kernel."""
+def _to_tokens(sample: torch.Tensor, repeat: int = 1, input_scale=None, step_ptr=None) -> torch.Tensor:
+    """[N, C, H, W] (any float dtype) -> bf16 [N*repeat, H, W, C] via the layout kernel. input_scale: fp32 device table
+    of the sampler's model-input scale, read at step_ptr[0] (scale_model_input of the sigma-space schedulers)."""
+    if input_scale is not None:
+        return ops.nchw_f32_to_nhwc_bf16_scaled(sample.float().contiguous(), input_scale, step_ptr, repeat=repeat)
     return ops.nchw_f32_to_nhwc_bf16(sample.float().contiguous(), repeat=repeat)
 
 
@@ -731,15 +734,18 @@ class UNet2DConditionModel(_ModelBase):
 
     @torch.no_grad()
     def forward_tokens(self, sample, timestep, encoder_hidden_states, cross_attention_kwargs=None,
-                       down_res=None, mid_res=None, timestep_table=None, out=None, sample_repeat: int = 1) -> torch.Tensor:
+                       down_res=None, mid_res=None, timestep_table=None, out=None, sample_repeat: int = 1,
+                       input_scale=None) -> torch.Tensor:
         """The hot path. Returns eps as fp32 NCHW (written by the conv_out kernel). sample_repeat=2 evaluates the
-        CFG-duplicated batch [sample, sample] without materialising the duplicate."""
+        CFG-duplicated batch [sample, sample] without materialising the duplicate. input_scale: per-step fp32 table of
+        the model-input scale, indexed by the step pointer of `timestep_table`."""
         kw = cross_attention_kwargs or {}
         pk = self._io_packed()
         NB = sample.shape[0] * sample_repeat
         ctx = self._ctx(encoder_hidden_states)
         temb_all = self.time_conditioning(NB, timestep, sample.device, timestep_table)
-        x = ops.conv3x3_direct(_to_tokens(sample, sample_repeat), pk["wi"], pk["bi"])
+        step_ptr = timestep_table[1] if timestep_table is not None else None
+        x = ops.conv3x3_direct(_to_tokens(sample, sample_repeat, input_scale, step_ptr), pk["wi"], pk["bi"])
         skips = [x]
         for blk in self.down_blocks:
             x, outs = blk.run(x, temb_all, ctx, kw)
@@ -868,14 +874,15 @@ class ControlNetModel(_ModelBase):
     def forward(self, sample, timestep, encoder_hidden_states, controlnet_cond, conditioning_scale: float = 1.0,
                 class_labels=None, timestep_cond=None, attention_mask=None, added_cond_kwargs=None,
                 cross_attention_kwargs=None, guess_mode: bool = False, return_dict: bool = True,
-                timestep_table=None, sample_repeat: int = 1):
+                timestep_table=None, sample_repeat: int = 1, input_scale=None):
         assert not guess_mode, "guess_mode is False in every reference script (SURVEY.md B14)"
         pk = self._cn_packed()
         NB = sample.shape[0] * sample_repeat
         ctx = self._ctx(encoder_hidden_states)
         temb_all = self.time_conditioning(NB, timestep, sample.device, timestep_table)
         cond = self.cond_embedding(controlnet_cond, NB)
-        x = ops.conv3x3_direct(_to_tokens(sample, sample_repeat), pk["wi"], pk["bi"], add=cond)
+        step_ptr = timestep_table[1] if timestep_table is not None else None
+        x = ops.conv3x3_direct(_to_tokens(sample, sample_repeat, input_scale, step_ptr), pk["wi"], pk["bi"], add=cond)
         skips = [x]
         for blk in self.down_blocks:
             x, outs = blk.run(x, temb_all, ctx, cross_attention_kwargs or {})

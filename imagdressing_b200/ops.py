@@ -351,6 +351,38 @@ def cfg_ddim_step(eps_cond: torch.Tensor, eps_uncond: Optional[torch.Tensor], gu
     return latents
 
 
+def nchw_f32_to_nhwc_bf16_scaled(x: torch.Tensor, scale_table: torch.Tensor, step_ptr: Optional[torch.Tensor], *,
+                                 repeat: int = 1, out=None) -> torch.Tensor:
+    """nchw_f32_to_nhwc_bf16 times scale_table[step_ptr[0]] (device-side read; step 0 without a step_ptr)."""
+    lib = _lib.load()
+    NB, C, H, W = x.shape
+    assert x.is_contiguous() and x.dtype == torch.float32 and scale_table.dtype == torch.float32
+    if out is None:
+        out = torch.empty(NB * repeat, H, W, C, device=x.device, dtype=BF16)
+    _lib.check(lib.imagd_nchw_f32_to_nhwc_bf16_scaled(x.data_ptr(), out.data_ptr(), NB, C, H, W, C, repeat,
+                                                      scale_table.data_ptr(), _ptr(step_ptr), _stream()),
+               "imagd_nchw_f32_to_nhwc_bf16_scaled")
+    return out
+
+
+def cfg_sampler_step(eps_cond: torch.Tensor, eps_uncond: Optional[torch.Tensor], guidance: float, latents: torch.Tensor,
+                     coef: torch.Tensor, step_ptr: torch.Tensor, *, history=None, step_noise=None, mask=None,
+                     image_latents=None, noise=None, blend_coef=None) -> torch.Tensor:
+    """In-place on `latents` (fp32 NCHW) and `history`. coef: fp32 [S, 6] rows {dx, de, cx, ce, ch, cz}
+    (include/imagd_b200.h); step_noise: fp32 [S, *latents.shape]; step_ptr: int32[2] device tensor {step, scratch}."""
+    lib = _lib.load()
+    NB, C, H, W = latents.shape
+    assert latents.dtype == torch.float32 and latents.is_contiguous() and eps_cond.dtype == torch.float32
+    assert step_ptr.dtype == torch.int32 and step_ptr.numel() >= 2 and coef.shape[-1] == 6
+    assert history is None or (history.shape == latents.shape and history.is_contiguous())
+    assert step_noise is None or (step_noise.shape[1:] == latents.shape and step_noise.is_contiguous())
+    rc = lib.imagd_cfg_sampler_step(eps_cond.data_ptr(), _ptr(eps_uncond), float(guidance), latents.data_ptr(),
+                                    _ptr(history), _ptr(step_noise), coef.data_ptr(), step_ptr.data_ptr(), _ptr(mask),
+                                    _ptr(image_latents), _ptr(noise), _ptr(blend_coef), NB, C, H * W, _stream())
+    _lib.check(rc, "imagd_cfg_sampler_step")
+    return latents
+
+
 def embed_tokens(ids: torch.Tensor, tok: torch.Tensor, pos: torch.Tensor) -> torch.Tensor:
     """ids int64 [B, T]; tok bf16 [V, C]; pos bf16 [>= T, C] -> bf16 [B, T, C] = tok[ids] + pos[:T]."""
     lib = _lib.load()

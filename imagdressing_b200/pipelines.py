@@ -259,8 +259,11 @@ class _DressingPipelineBase:
              # IP-Adapter
              face_tokens=None, face_null_tokens=None,
              # inpainting
-             mask=None, image_latents=None, strength=1.0, noise=None):
+             mask=None, image_latents=None, strength=1.0, noise=None, latents_scaled=False):
+        """latents_scaled: `latents` is already the sampler's start (the inpainting pipeline builds it as
+        noise * init_noise_sigma or add_noise(image_latents, noise, t_start)), so it is not rescaled here."""
         device = self._execution_device
+        scheduler = self.scheduler
         self._cross_attention_kwargs = cross_attention_kwargs
         self._clip_skip = clip_skip
         if guidance_scale <= 1.0:
@@ -279,14 +282,23 @@ class _DressingPipelineBase:
             negative_prompt_embeds = torch.cat(
                 [negative_prompt_embeds, fn.to(prompt_embeds).expand(negative_prompt_embeds.shape[0], -1, -1)], 1)
 
-        self.scheduler.set_timesteps(num_inference_steps, device=device)
-        timesteps = self.scheduler.timesteps
+        scheduler.set_timesteps(num_inference_steps, device=device)
+        timesteps = scheduler.timesteps
         if self._inpaint and strength < 1.0:
             init = min(int(num_inference_steps * strength), num_inference_steps)
             timesteps = timesteps[max(num_inference_steps - init, 0):]
 
-        latents = self.prepare_latents(n, self.unet.config.in_channels, width, height, torch.float32, device, generator,
-                                       latents)
+        if latents_scaled:
+            latents = latents.to(device=device, dtype=torch.float32)
+        else:
+            latents = self.prepare_latents(n, self.unet.config.in_channels, width, height, torch.float32, device,
+                                           generator, latents)
+        step_noise = None
+        if getattr(scheduler, "_needs_noise", False):
+            # Euler-ancestral: the reference loop's step() draws one latents-shaped tensor per step from `generator`,
+            # in step order after prepare_latents; drawn here in the same order and staged for the captured graph
+            step_noise = torch.stack([randn_tensor(latents.shape, generator=generator, device=device)
+                                      for _ in range(len(timesteps))])
         gtok = self._garment_tokens(ref_clip_image, garment_tokens, device, prompt_embeds.dtype, control_pe)
         if gtok.shape[0] != n:
             gtok = gtok.expand(n, -1, -1)
@@ -302,7 +314,7 @@ class _DressingPipelineBase:
             control_keep=keep,
             control_cond=control_image, control_prompt_embeds=control_pe, control_negative_embeds=control_ne,
             control_scale=controlnet_conditioning_scale, mask=mask, image_latents=image_latents, noise=noise,
-            callback=callback)
+            callback=callback, scheduler=scheduler, step_noise=step_noise)
         image = self._decode(out, output_type, generator)
         if not return_dict:
             return (image, None)
@@ -499,7 +511,8 @@ class IMAGDressing_v1_ControlNetInpaint(IMAGDressing_v1_ControlNet):
         if mask_latents.shape[0] != n:
             mask_latents = mask_latents.expand(n, -1, -1, -1)
         noise = randn_tensor(image_latents.shape, generator=generator, device=dev) if latents is None else latents.to(dev)
-        # is_strength_max: pure noise start; else add_noise(image_latents, noise, t_start) (inherited prepare_latents)
+        # is_strength_max: pure noise start scaled by init_noise_sigma; else add_noise(image_latents, noise, t_start),
+        # not rescaled (inherited prepare_latents); _run takes the start as is
         self.scheduler.set_timesteps(num_inference_steps, device=dev)
         ts = self.scheduler.timesteps
         if strength < 1.0:
@@ -517,4 +530,4 @@ class IMAGDressing_v1_ControlNetInpaint(IMAGDressing_v1_ControlNet):
                          ref_image_latents=ref_image_latents, control_image=ctrl,
                          controlnet_conditioning_scale=float(controlnet_conditioning_scale), mask=mask_latents,
                          image_latents=image_latents, strength=strength, noise=noise, control_guidance_start=cg_start,
-                         control_guidance_end=cg_end)
+                         control_guidance_end=cg_end, latents_scaled=True)

@@ -185,6 +185,11 @@ int imagd_conv3x3_direct_bf16(const void* x, int NB, int H, int W, int Cin, cons
  * dressing_sd/pipelines/IMAGDressing_v1_pipeline.py:483-485) in the same pass. */
 int imagd_nchw_f32_to_nhwc_bf16(const float* x, void* y, int NB, int C, int H, int W, int Cpad, int repeat,
                                 imagd_stream stream);
+/* The same layout with every value multiplied by scale_table[step_ptr ? *step_ptr : 0]: the model-input scaling
+ * x / sqrt(sigma_i^2 + 1) of the sigma-space samplers (EulerDiscreteScheduler.scale_model_input, diffusers-0.24),
+ * read on the device so a captured step graph walks the table. */
+int imagd_nchw_f32_to_nhwc_bf16_scaled(const float* x, void* y, int NB, int C, int H, int W, int Cpad, int repeat,
+                                       const float* scale_table, const int32_t* step_ptr, imagd_stream stream);
 
 /* ---- CLIP encoder front ends (SURVEY.md 8f row 3; transformers CLIPTextModel / CLIPVisionModelWithProjection, reference
  * call sites inference_IMAGdressing.py:44-49, IMAGDressing_v1_pipeline.py:396-415) ---- */
@@ -225,6 +230,19 @@ int imagd_cfg_ddim_step(const float* eps_cond, const float* eps_uncond, float gu
                         const float* coef, int32_t* step_ptr, const float* mask, const float* image_latents,
                         const float* noise, const float* blend_coef, int NB, int C, int HW,
                         imagd_stream stream);
+/* Classifier-free guidance + one step of a multistep sampler (DPMSolverMultistepScheduler dpmsolver++ order 1/2,
+ * EulerDiscreteScheduler, EulerAncestralDiscreteScheduler; diffusers-0.24), optionally + the inpainting blend.
+ * coef: device array [n_steps, 6], row = {dx, de, cx, ce, ch, cz}; per element, with eps the CFG-combined output:
+ *   D  = dx x + de eps                         (the data prediction of this step)
+ *   x' = cx x + ce eps + ch H + cz z[step]     (H: history, the previous step's D; z: this step's noise)
+ *   if history: H = D (after reading it)
+ *   if mask: x' = (1-mask) * (blend[0] img + blend[1] noise) + mask * x'
+ * history: fp32 [NB,C,h,w] or NULL; step_noise: fp32 [n_steps,NB,C,h,w] or NULL. A zero ch / cz skips reading its
+ * operand. step_ptr and blend_coef as for imagd_cfg_ddim_step (the kernel advances the step counter). */
+int imagd_cfg_sampler_step(const float* eps_cond, const float* eps_uncond, float guidance, float* latents,
+                           float* history, const float* step_noise, const float* coef, int32_t* step_ptr,
+                           const float* mask, const float* image_latents, const float* noise, const float* blend_coef,
+                           int NB, int C, int HW, imagd_stream stream);
 
 /* ================================================================================================================
  * Training step (SURVEY.md 8 row a13; reference train.py:255-281 SDModel.forward, :573-605 loss + backward, :386-398 AdamW).
