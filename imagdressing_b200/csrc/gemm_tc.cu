@@ -612,10 +612,20 @@ static int ensure_scratch(float** ws, unsigned int** counters, cudaStream_t stre
 
 // ---- tile / pipeline-depth / split-K choice --------------------------------------------------------------------
 // Variants: N tile 64 / 128 / 160 / 256 with a "shallow" (2-4 stages) or "deep" (4-8 stages, ~190 KB) operand ring. Every
-// variant runs one CTA per SM; the shared-memory footprint is max(ring, 128 x (4 BN + 16) bytes of accumulator staging)
-// plus the epilogue vectors (about 96-200 KB). Deep rings keep more bytes in flight for grids of at most one wave, where
-// each CTA is bound by the latency of its own TMA ring; split-K serves the deep UNet levels whose output has only a
-// handful of tiles. The thresholds below are a rule of thumb in units of the 132 SMs, not tuned by measurement on H100.
+// variant runs one CTA per SM (the register file allows no second one); the shared-memory footprint is max(ring,
+// 128 x (4 BN + 16) bytes of accumulator staging) plus the epilogue vectors (about 96-200 KB).
+//
+// Measured on an H100 80GB HBM3 (SXM, 400 W power limit, 1980 MHz max SM clock) with tools/gemm_bench.py over the 92
+// launch keys of a denoising step at batch 1 and 8, every variant timed in isolation:
+//   - the deep ring is faster than the shallow one for nearly every key, one wave or many;
+//   - a CTA spends about a constant time per k-block that grows with the operand bytes of the k-block (16 KB of A plus
+//     BN x 128 B of B), roughly 75 GB/s per SM: 0.32 / 0.45 / 0.50 / 0.65 us for BN = 64 / 128 / 160 / 256;
+//   - the chip-wide rate is not the limit: variants reach 6.6-7.8 TB/s of modelled L2 -> shared-memory operand
+//     traffic, and the slow launches of the old rule (~4-5 TB/s) lost their time to partly filled last waves.
+// So the rule minimises  waves x (t_wave(BN) + k-blocks per CTA x t_kb(BN)) + t_split x (MB of split-K partials)  with
+// waves = ceil(CTAs / 132), t_kb / t_wave (prologue + epilogue) fitted by least squares to those timings. With it the
+// step's GEMM + conv launches take 4.6 ms instead of 6.2 ms at batch 1 and 28.4 ms instead of 32.7 ms at batch 8
+// (sum of the isolated launch times, same card).
 struct GemmCfg {
     int bn, stages, splits;
 };
@@ -623,21 +633,33 @@ struct GemmCfg {
 static int shallow_stages(int bn) { return bn == 64 ? 4 : (bn == 256 ? 2 : 3); }
 static int deep_stages(int bn) { return bn == 64 ? 8 : (bn == 128 ? 6 : (bn == 160 ? 5 : 4)); }
 
-static GemmCfg choose_cfg(int m_tiles, int N, int kb_total, bool geglu) {
-    auto ctas = [&](int bn) { return static_cast<int64_t>(m_tiles) * ((N + bn - 1) / bn); };
-    if (geglu) return {128, ctas(128) > kNumSms ? 3 : 6, 1};
-    if (ctas(160) >= 3 * kNumSms) return {160, 3, 1};  // many waves: widest 2-CTA/SM tile
-    int bn = 64;
-    if (ctas(160) >= kNumSms && ctas(160) <= 2 * kNumSms && (N % 160 == 0 || N > 640)) bn = 160;
-    else if (ctas(128) >= kNumSms) bn = 128;
-    int splits = 1;
-    if (ctas(bn) < kNumSms * 2 / 3 && kb_total >= 60) {
-        splits = static_cast<int>((kNumSms + ctas(bn) - 1) / ctas(bn));
-        splits = std::min(splits, std::min(6, kb_total / 30));
-        splits = std::max(splits, 1);
+static GemmCfg choose_cfg(int m_tiles, int N, int kb_total, bool geglu, bool allow_split) {
+    constexpr int kBn[4] = {64, 128, 160, 256};
+    constexpr double kWaveUs[4] = {3.76, 5.31, 7.34, 10.18};  // per wave: prologue, pipeline fill, epilogue
+    constexpr double kKbUs[4] = {0.324, 0.454, 0.496, 0.648};  // per k-block of one CTA, deep ring
+    constexpr double kSplitUsPerMB = 1.94;                     // fp32 partials written and reduced
+    GemmCfg best{128, deep_stages(128), 1};
+    double best_us = 1e30;
+    for (int i = 0; i < 4; ++i) {
+        const int bn = kBn[i];
+        if (geglu && bn != 128) continue;  // the GEGLU epilogue pairs the value / gate halves of a 128-wide tile
+        const int64_t tiles = static_cast<int64_t>(m_tiles) * ((N + bn - 1) / bn);
+        for (int splits = 1; splits <= 6; ++splits) {
+            // split-K for long K only (>= 30 k-blocks per split) and within the scratch (kWsBytes, kMaxTilesSplit)
+            if (splits > 1 && (!allow_split || kb_total / splits < 30 || tiles > kMaxTilesSplit ||
+                               static_cast<size_t>(tiles * splits) * 128 * bn * 4 > kWsBytes))
+                continue;
+            const int64_t waves = (tiles * splits + kNumSms - 1) / kNumSms;
+            const int kb = (kb_total + splits - 1) / splits;
+            const double part_mb = splits > 1 ? static_cast<double>(tiles * splits) * 128 * bn * 4 / 1e6 : 0.0;
+            const double us = static_cast<double>(waves) * (kWaveUs[i] + kb * kKbUs[i]) + kSplitUsPerMB * part_mb;
+            if (us < best_us) {
+                best_us = us;
+                best = {bn, deep_stages(bn), splits};
+            }
+        }
     }
-    const bool deep = ctas(bn) * splits <= kNumSms;
-    return {bn, deep ? deep_stages(bn) : shallow_stages(bn), splits};
+    return best;
 }
 
 template <int BLOCK_N, int STAGES, int EPI, int LNM = 0>
@@ -686,7 +708,7 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const Gem
 static int g_force_bn = 0, g_force_stages = 0, g_force_splits = 0;  // test hooks (imagd_gemm_debug_force)
 static int g_log_on = 0;
 static unsigned long long* g_dbg_timeline = nullptr;  // imagd_gemm_debug_timeline
-static std::vector<std::string> g_log;  // unique problem keys seen while logging (tools/gemm_sweep.py)
+static std::vector<std::pair<std::string, int>> g_log;  // unique keys seen while logging, launch counts (tools/gemm_bench.py)
 
 static int run_gemm_like(const void* A, int64_t lda, int NB, int H, int W, int Cin, int taps, const void* Wt,
                          int64_t ldw, void* D, int64_t ldd, int N, const imagd_epilogue* ep_in, cudaStream_t stream,
@@ -743,19 +765,13 @@ static int run_gemm_like(const void* A, int64_t lda, int NB, int H, int W, int C
     const int m_tiles = static_cast<int>(m_tiles64);
     const int kb_total = taps * p.kb_per_tap;
 
-    GemmCfg cfg = choose_cfg(m_tiles, N, kb_total, geglu);
+    GemmCfg cfg = choose_cfg(m_tiles, N, kb_total, geglu, !ups_mode);
     if (g_force_bn) {
         cfg.bn = geglu ? 128 : g_force_bn;
         cfg.stages = g_force_stages ? g_force_stages : shallow_stages(cfg.bn);
         if (cfg.stages != shallow_stages(cfg.bn) && cfg.stages != deep_stages(cfg.bn)) cfg.stages = shallow_stages(cfg.bn);
     }
     if (g_force_splits && !geglu) cfg.splits = std::min(g_force_splits, kb_total);
-    if (g_log_on) {
-        char key[160];
-        snprintf(key, sizeof(key), "%d %d %d %d %d %d %d %d %d %d", taps, NB, H, W, Cin, N, geglu ? 1 : 0, m_tiles,
-                 kb_total, ep.out_fp32);
-        if (std::find(g_log.begin(), g_log.end(), key) == g_log.end()) g_log.push_back(key);
-    }
     IMAGD_CHECK_ARG(!ep.row_stats_out || ep.stats_ld >= (N + cfg.bn - 1) / cfg.bn,
                     "gemm: stats_ld=%lld is smaller than the %d N tiles of this launch (imagd_gemm_tile_count_n)",
                     (long long)ep.stats_ld, (N + cfg.bn - 1) / cfg.bn);
@@ -765,6 +781,14 @@ static int run_gemm_like(const void* A, int64_t lda, int NB, int H, int W, int C
     p.splits = cfg.splits;
     p.kb_per_split = (kb_total + cfg.splits - 1) / cfg.splits;
     p.splits = (kb_total + p.kb_per_split - 1) / p.kb_per_split;  // no empty splits
+    if (g_log_on) {  // problem key | the configuration this launch runs
+        char key[192];
+        snprintf(key, sizeof(key), "%d %d %d %d %d %d %d %d %d %d | %d %d %d", taps, NB, H, W, Cin, N, geglu ? 1 : 0,
+                 m_tiles, kb_total, ep.out_fp32, cfg.bn, cfg.stages, p.splits);
+        auto it = std::find_if(g_log.begin(), g_log.end(), [&](const auto& e) { return e.first == key; });
+        if (it == g_log.end()) g_log.emplace_back(key, 1);
+        else ++it->second;
+    }
     p.ws = nullptr;
     p.counters = nullptr;
     p.dbg = g_dbg_timeline;
@@ -836,7 +860,7 @@ int imagd_gemm_debug_log(int enable, char* out, int out_bytes) {
     }
     if (out && out_bytes > 0) {
         std::string all;
-        for (const auto& k : imagd::g_log) all += k + "\n";
+        for (const auto& k : imagd::g_log) all += k.first + " | " + std::to_string(k.second) + "\n";
         IMAGD_CHECK_ARG(static_cast<int>(all.size()) < out_bytes, "debug_log: buffer too small (%d needed)",
                         static_cast<int>(all.size()) + 1);
         memcpy(out, all.c_str(), all.size() + 1);
@@ -860,7 +884,7 @@ int imagd_gemm_tile_count_n(int M, int N, int K) {
     int bw = 1, bh = 1, bn = 1;
     choose_pixel_box(M, 1, 1, &bw, &bh, &bn);
     const int m_tiles = ((M + bw - 1) / bw);
-    GemmCfg cfg = choose_cfg(m_tiles, N, (K + kBlockK - 1) / kBlockK, false);
+    GemmCfg cfg = choose_cfg(m_tiles, N, (K + kBlockK - 1) / kBlockK, false, true);
     if (g_force_bn) cfg.bn = g_force_bn;
     return (N + cfg.bn - 1) / cfg.bn;
 }

@@ -81,8 +81,9 @@ int imagd_gemm_bf16(const void* A, int64_t lda, const void* W, int64_t ldw, void
 /* Test / tuning hooks. debug_force: force the N tile (0 = automatic; 64 / 128 / 160 / 256), the TMA ring depth
  * (0 = the shallow two-CTAs-per-SM variant) and the split-K factor (0 = automatic) of the next imagd_gemm_bf16 /
  * imagd_conv3x3_bf16 calls, so the parity tests cover every kernel variant. debug_log: enable = 1 starts recording
- * the distinct problems issued ("taps NB H W Cin N geglu m_tiles kb_total out_fp32" per line), 0 stops, -1 leaves
- * the state; when `out` is given the recorded lines are copied there. Returns the number of lines. */
+ * the distinct launches issued ("taps NB H W Cin N geglu m_tiles kb_total out_fp32 | block_n stages splits | count"
+ * per line: the problem, the configuration it ran with, how many times), 0 stops, -1 leaves the state; when `out` is
+ * given the recorded lines are copied there. Returns the number of lines. */
 int imagd_gemm_debug_force(int block_n, int stages, int splits);
 /* r2-prep: Upsample2D (nearest 2x) + its 3x3 conv in one implicit GEMM over the LOW-resolution input: four 2x2 "phase"
  * convolutions (output pixel (2y+py, 2x+px) sees input rows {y+py-1, y+py} and columns {x+px-1, x+px}); Wt is the
