@@ -51,7 +51,7 @@ static void resolve_encode() {
 }
 
 int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                   const uint32_t* box) {
+                   const uint32_t* box, CUtensorMapSwizzle swizzle) {
     std::call_once(g_encode_once, resolve_encode);
     if (!g_encode) {
         set_error("cuTensorMapEncodeTiled not available (no CUDA driver?)");
@@ -80,7 +80,7 @@ int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t*
     }
     CUresult r = g_encode(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, static_cast<cuuint32_t>(rank),
                           const_cast<void*>(base), gdim, gstr, bdim, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                          CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                          swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                           CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) {
         set_error("cuTensorMapEncodeTiled failed: CUresult %d (rank %d dims %llu,%llu,%llu,%llu box %u,%u,%u,%u)",

@@ -50,10 +50,10 @@ int cuda_fail(cudaError_t e, const char* what);
         if (e__ != cudaSuccess) return ::imagd::cuda_fail(e__, name);  \
     } while (0)
 
-// Encode a tiled bf16 TMA descriptor (SWIZZLE_128B, OOB zero fill). dims/strides innermost first;
+// Encode a tiled bf16 TMA descriptor (SWIZZLE_128B unless given, OOB zero fill). dims/strides innermost first;
 // strides_bytes has rank-1 entries (stride of dim 1..rank-1). Returns IMAGD_OK or an error code.
 int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                   const uint32_t* box);
+                   const uint32_t* box, CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B);
 
 // Launch, optionally with the programmatic-dependent-launch attribute (IMAGD_PDL=1 in the environment enables it).
 bool pdl_enabled();

@@ -8,9 +8,9 @@
 // kernel with one tap and a [K, M, 1, 1] view.
 //
 // CTA = 128 output pixels x BLOCK_N output channels: a TMA producer warp feeds a STAGES-deep ring of 128B-swizzled
-// A / B tiles, two warpgroups accumulate 64 rows each with wgmma in registers, and the accumulator tile is handed to
-// the epilogue through shared memory (bias / time-embedding row vector / activation / residual -> bf16 stores).
-// One CTA runs per SM (288 threads, up to 168 registers each, 96-200 KB of shared memory).
+// A / B tiles (then the residual tile), two warpgroups accumulate 64 rows each with wgmma in registers and apply the
+// epilogue (bias / time-embedding row vector / activation / residual) to their own fragments; the bf16 tile leaves by
+// TMA stores. One CTA runs per SM (288 threads, 96-200 KB of shared memory).
 #include <algorithm>
 #include <cstring>
 #include <mutex>
@@ -46,6 +46,8 @@ struct GemmParams {
     unsigned long long* dbg;
     int ups_n_tiles;  // LNM == 3: N tiles per phase (gridDim.y = 4 * ups_n_tiles)
     int pdl_late;     // 1: release the dependent kernel when the accumulator is complete instead of at kernel entry
+    int res_tma;      // 1: the residual is read through tmR (any epilogue but GEGLU)
+    int store_tma;    // 1: the bf16 output is written through tmD (all but fp32 outputs and the upsample-phase conv)
 };
 
 __device__ __forceinline__ void dbg_mark(const GemmParams& p, int slot) {
@@ -59,39 +61,48 @@ constexpr int kBlockM = 128;
 constexpr int kBlockK = 64;
 constexpr int kABytes = kBlockM * kBlockK * 2;  // 16 KB
 constexpr int kGemmThreads = 288;               // two consumer warpgroups + one producer warp
+// The bf16 residual (in) and the bf16 output (out) tiles pass through shared memory in chunks of 32 columns x 128 rows:
+// TMA boxes of (32 channels, bw, bh, bn) pixels, 64-byte rows in the 64-byte swizzle (conflict-free fragment-order access)
+constexpr int kEpiCols = 32;
+constexpr int kEpiChunkBytes = kBlockM * kEpiCols * 2;  // 8 KB
+constexpr int kRowGroups = 4;  // row-vector groups (samples) one tile may span with its row vector staged in shared memory
 
 template <int BLOCK_N, int STAGES>
 struct GemmSmem {
     static constexpr int kBBytes = BLOCK_N * kBlockK * 2;
     static constexpr int kStageBytes = kABytes + kBBytes;
     static constexpr int kRing = STAGES * kStageBytes;
-    // after the mainloop the fp32 accumulator tile is staged row by row over the idle operand ring: one row per epilogue
-    // thread, +16 bytes so that the float4 reads of eight consecutive rows hit eight bank groups
-    static constexpr int kAccRowBytes = BLOCK_N * 4 + 16;
-    static constexpr int kAccBytes = kBlockM * kAccRowBytes;
-    static constexpr int kBarOffset = (kRing > kAccBytes ? kRing : kAccBytes);
-    static constexpr int kVecOffset = (kBarOffset + (2 * STAGES) * 8 + 16 + 15) & ~15;  // float4 reads
-    // epilogue vectors staged once per CTA: bias[BLOCK_N] | row vector[BLOCK_N] (when the tile lies in one row group)
-    static constexpr int kTotal = kVecOffset + 2 * BLOCK_N * 4;
+    // epilogue chunk c lives in the ring stage that producer iteration nk + c / kChunksPerStage would fill
+    static constexpr int kChunksPerStage = kStageBytes / kEpiChunkBytes;
+    static_assert(BLOCK_N / kEpiCols <= STAGES * kChunksPerStage, "epilogue tile does not fit the ring");
+    static constexpr int kBarOffset = kRing;
+    // full[STAGES] | empty[STAGES] | residual | split-K flag
+    static constexpr int kVecOffset = (kBarOffset + (2 * STAGES + 1) * 8 + 16 + 15) & ~15;
+    // epilogue vectors staged once per CTA: bias[BLOCK_N] | row vector[kRowGroups][BLOCK_N] (LayerNorm consumer: column sums)
+    static constexpr int kTotal = kVecOffset + (1 + kRowGroups) * BLOCK_N * 4;
 };
 
-// LINEAR = the epilogue has no activation and writes bf16 (every conv and most linears of the UNet): straight-line,
-// branch-free column loop. !LINEAR = the generic epilogue (SiLU / GELU / GEGLU / fp32 output).
-// EPI: 0 generic, 1 LINEAR, 2 LINEAR with the output row staged in shared memory (in the thread's own accumulator row,
-// behind the columns it has already read) and written by one bulk copy per row instead of 16-byte stores.
+// Byte offset of (tile row r, even chunk column cl) in an epilogue chunk: rows of 64 bytes, TMA SWIZZLE_64B (16-byte unit
+// bits [4, 6) XOR address bits [7, 9)). The eight rows a warp touches per access land in eight distinct 16-byte units.
+__device__ __forceinline__ int epi_offset(int r, int cl) { return r * 64 + ((cl * 2) ^ (((r >> 1) & 3) << 4)); }
+
+// LINEAR = the epilogue has no activation and writes bf16 (every conv and most linears of the UNet); !LINEAR = the
+// generic epilogue (SiLU / GELU / quick-GELU / GEGLU / fp32 output).
 // LNM: LayerNorm folding (see include/imagd_b200.h): 0 off, 1 producer (emit per-row {sum, sum of squares} of the rounded
-// outputs, one slot per N tile), 2 consumer (apply rstd * (alpha * acc - mean * colsum) + bias).
+// outputs, one slot per N tile), 2 consumer (apply rstd * (alpha * acc - mean * colsum) + bias), 3 upsample-phase conv.
 //
 // CTA = 128 output pixels x BLOCK_N output channels, 288 threads:
-//   warps 0-3  warpgroup 0: wgmma on accumulator rows 0-63, then the epilogue (thread = tile row)
-//   warps 4-7  warpgroup 1: wgmma on accumulator rows 64-127
-//   warp 8     TMA producer (one elected lane; STAGES-deep smem ring, full / empty mbarriers)
-template <int BLOCK_N, int STAGES, int EPI, int LNM>
+//   warps 0-3  warpgroup 0: wgmma on accumulator rows 0-63, then the epilogue of those rows from registers
+//   warps 4-7  warpgroup 1: the same for rows 64-127
+//   warp 8     TMA producer (one elected lane; STAGES-deep smem ring, full / empty mbarriers; then the residual tile)
+// The epilogue applies bias / row vector / activation / residual to the accumulator fragments, stages the bf16 tile over
+// the idle ring and writes it with TMA tile stores (the tensor map clips ragged M / N edges). fp32 outputs and the
+// upsample-phase conv store straight from the fragments.
+template <int BLOCK_N, int STAGES, bool LINEAR, int LNM>
 __global__ void __launch_bounds__(kGemmThreads, 1)
-gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
+gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+               const __grid_constant__ CUtensorMap tmR, const __grid_constant__ CUtensorMap tmD, const GemmParams p) {
     using L = GemmSmem<BLOCK_N, STAGES>;
-    constexpr bool LINEAR = EPI != 0;
-    constexpr bool BULK = EPI == 2;
     constexpr bool LN_PRODUCE = LNM == 1;
     constexpr bool LN_CONSUME = LNM == 2;
     // LNM == 3: nearest-2x upsample + 3x3 conv as four 2x2 "phase" convs on the LOW-resolution input (2.25x fewer MACs,
@@ -99,13 +110,15 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     // pixel (y + py - 1 + ty, x + px - 1 + tx); the weight matrix is [4 * N, 4 * Cin] (phase-major rows, tap-major
     // columns); output pixel (2y + py, 2x + px) of a [NB, 2H, 2W, N] tensor.
     constexpr bool UPS = LNM == 3;
+    constexpr int kResChunks = BLOCK_N / kEpiCols;
     static_assert(!LN_PRODUCE || LINEAR, "row statistics are emitted by the LINEAR epilogue only");
     static_assert(BLOCK_N % 64 == 0 || BLOCK_N == 160, "wgmma N tile");
     extern __shared__ __align__(1024) uint8_t smem[];  // SWIZZLE_128B tiles need 1024-byte alignment
     if (threadIdx.x == 0 && (smem_u32(smem) & 1023u) != 0) __trap();  // (no printf: see mbar_wait_quiet)
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::kBarOffset);
     uint64_t* empty_bar = full_bar + STAGES;
-    uint32_t* flag_slot = reinterpret_cast<uint32_t*>(empty_bar + STAGES);
+    uint64_t* res_bar = empty_bar + STAGES;
+    uint32_t* flag_slot = reinterpret_cast<uint32_t*>(res_bar + 1);
     float* s_bias = reinterpret_cast<float*>(smem + L::kVecOffset);
     float* s_rowvec = s_bias + BLOCK_N;
 
@@ -134,6 +147,15 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     const int total_kb = p.taps * p.kb_per_tap;
     const int kb_begin = blockIdx.z * p.kb_per_split;
     const int nk = min(total_kb, kb_begin + p.kb_per_split) - kb_begin;  // >= 1 (host guarantees)
+    const int col_base = n_blk * BLOCK_N;
+    auto epi_chunk = [&](int c) {
+        return smem + ((nk + c / L::kChunksPerStage) % STAGES) * L::kStageBytes + (c % L::kChunksPerStage) * kEpiChunkBytes;
+    };
+    auto load_residual = [&]() {  // one elected thread; completes on res_bar
+        mbar_arrive_expect_tx(res_bar, kResChunks * kEpiChunkBytes);
+#pragma unroll 1
+        for (int c = 0; c < kResChunks; ++c) tma_load_4d(epi_chunk(c), &tmR, res_bar, col_base + c * kEpiCols, x0, y0, n0);
+    };
 
     if (threadIdx.x == 0) {
         tma_prefetch_desc(&tmA);
@@ -142,6 +164,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             mbar_init(&full_bar[i], 1);
             mbar_init(&empty_bar[i], 2);  // one arrival per consumer warpgroup
         }
+        mbar_init(res_bar, 1);
         fence_barrier_init();
     }
     __syncthreads();
@@ -172,56 +195,73 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                 tma_load_2d(sb, &tmB, &full_bar[stage], tap * p.cin + kc * kBlockK,
                             (UPS ? ups_phase * p.N : 0) + n_blk * BLOCK_N);
             }
+            // the residual tile goes to the stages of iterations nk, nk + 1, ...: free from the start when nk < STAGES,
+            // otherwise as soon as the consumers release them at the end of the K loop. (Split-K: the last arriver loads it.)
+            if (p.res_tma && p.splits == 1) {
+                for (int c = 0; c < kResChunks; c += L::kChunksPerStage) {
+                    const int v = nk + c / L::kChunksPerStage;
+                    mbar_wait_quiet(&empty_bar[v % STAGES], ((v / STAGES) & 1) ^ 1);
+                }
+                load_residual();
+            }
         }
         return;
     }
 
     const int wg = warp >> 2;  // consumer warpgroup: accumulator rows [64 wg, 64 wg + 64)
+    const int ct = threadIdx.x;  // consumer thread 0..255
     const imagd_epilogue& ep = p.ep;
-    const int col_base = n_blk * BLOCK_N;
-    // ---- epilogue preparation (warpgroup 0, before the mainloop): stage the per-column vectors in shared memory (every
-    // row of the tile reads the same bias; the row vector too when the whole tile lies in one row group, i.e. one sample)
-    const int r = threadIdx.x;  // warpgroup 0: tile-local pixel
-    const int x = x0 + r % p.bw;
-    const int y = y0 + (r / p.bw) % p.bh;
-    const int n = n0 + r / (p.bw * p.bh);
-    const bool row_ok = (x < p.W) && (y < p.H) && (n < p.NB);
-    const int64_t pix = UPS ? (static_cast<int64_t>(n) * (2 * p.H) + (2 * y + (ups_phase >> 1))) * (2 * p.W) +
-                                  (2 * x + (ups_phase & 1))
-                            : (static_cast<int64_t>(n) * p.H + y) * p.W + x;
-    const float* rowvec = nullptr;  // per-thread global fallback (tile spans several row groups)
-    bool rowvec_shared = false;
-    float ln_mean = 0.f, ln_rstd = 0.f;
-    if (wg == 0) {
-        if (ep.rowvec != nullptr) {
-            const int xl = min(x0 + p.bw, p.W) - 1, yl = min(y0 + p.bh, p.H) - 1, nl = min(n0 + p.bn, p.NB) - 1;
-            const int64_t pix_first = (static_cast<int64_t>(n0) * p.H + y0) * p.W + x0;
-            const int64_t pix_last = (static_cast<int64_t>(nl) * p.H + yl) * p.W + xl;
-            const int64_t g_first = pix_first / ep.rows_per_group;
-            rowvec_shared = g_first == pix_last / ep.rows_per_group;
-            if (rowvec_shared) {
-                const float* src = ep.rowvec + g_first * ep.rowvec_ld;
-                for (int c = threadIdx.x; c < BLOCK_N; c += 128)
-                    s_rowvec[c] = (col_base + c < p.N) ? __ldg(src + col_base + c) : 0.f;
-            } else if (row_ok) {
-                rowvec = ep.rowvec + (pix / ep.rows_per_group) * ep.rowvec_ld;
+    // wgmma m64nN accumulator layout: warp w of the warpgroup holds rows 16 w + lane / 4 (+ 8), columns 8 j + 2 (lane % 4)
+    // (+ 1); acc[4 j + 2 h + e] is (row frow + 8 h, column 8 j + 2 (lane % 4) + e)
+    const int quad = lane & 3;
+    const int frow = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    auto row_at = [&](int h, int64_t& pix) {  // output pixel of fragment row h; false outside the image
+        const int r = frow + 8 * h;
+        const int x = x0 + r % p.bw;
+        const int y = y0 + (r / p.bw) % p.bh;
+        const int n = n0 + r / (p.bw * p.bh);
+        pix = UPS ? (static_cast<int64_t>(n) * (2 * p.H) + (2 * y + (ups_phase >> 1))) * (2 * p.W) + (2 * x + (ups_phase & 1))
+                  : (static_cast<int64_t>(n) * p.H + y) * p.W + x;
+        return (x < p.W) && (y < p.H) && (n < p.NB);
+    };
+    int64_t pix[2];
+    bool row_ok[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) row_ok[h] = row_at(h, pix[h]);
+    // ---- epilogue preparation (before the mainloop): stage the per-column vectors in shared memory. The row vector is
+    // staged per row group (sample) when the tile spans at most kRowGroups of them; otherwise each row reads it from
+    // global memory. Without a row vector the LINEAR epilogue adds the zeroed slot, as it always adds bias and row vector.
+    const float* rowvec[2] = {s_rowvec, s_rowvec};
+    float ln_mean[2] = {0.f, 0.f}, ln_rstd[2] = {0.f, 0.f};
+    if (LN_CONSUME) {  // the row-vector slot carries the folded weight's column sums instead
+        for (int c = ct; c < BLOCK_N; c += 256) s_rowvec[c] = (col_base + c < p.N) ? __ldg(ep.colsum + col_base + c) : 0.f;
+    } else if (ep.rowvec != nullptr) {
+        const int xl = min(x0 + p.bw, p.W) - 1, yl = min(y0 + p.bh, p.H) - 1, nl = min(n0 + p.bn, p.NB) - 1;
+        const int64_t g_first = ((static_cast<int64_t>(n0) * p.H + y0) * p.W + x0) / ep.rows_per_group;
+        const int64_t g_last = ((static_cast<int64_t>(nl) * p.H + yl) * p.W + xl) / ep.rows_per_group;
+        const bool staged = g_last - g_first < kRowGroups;
+        if (staged) {
+            for (int i = ct; i < (g_last - g_first + 1) * BLOCK_N; i += 256) {
+                const int c = i % BLOCK_N;
+                s_rowvec[i] = (col_base + c < p.N) ? __ldg(ep.rowvec + (g_first + i / BLOCK_N) * ep.rowvec_ld + col_base + c)
+                                                   : 0.f;
             }
         }
-        if constexpr (LN_CONSUME) {  // the row-vector slot carries the folded weight's column sums instead
-            for (int c = threadIdx.x; c < BLOCK_N; c += 128)
-                s_rowvec[c] = (col_base + c < p.N) ? __ldg(ep.colsum + col_base + c) : 0.f;
-        } else if (LINEAR && !rowvec_shared) {  // the straight-line loop always adds the staged vectors: absent = zeros
-            for (int c = threadIdx.x; c < BLOCK_N; c += 128) s_rowvec[c] = 0.f;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int64_t g = pix[h] / ep.rows_per_group;
+            if (row_ok[h]) rowvec[h] = staged ? s_rowvec + (g - g_first) * BLOCK_N : ep.rowvec + g * ep.rowvec_ld + col_base;
         }
-        if (ep.bias != nullptr) {
-            for (int c = threadIdx.x; c < BLOCK_N; c += 128)
-                s_bias[c] = (col_base + c < p.N) ? __ldg(ep.bias + col_base + c) : 0.f;
-        } else if (LINEAR) {
-            for (int c = threadIdx.x; c < BLOCK_N; c += 128) s_bias[c] = 0.f;
-        }
-        if constexpr (LN_CONSUME) {
-            if (row_ok) {  // fixed-order fold of the producer's per-tile partials -> mean / rstd of my row of A
-                const float2* sp = reinterpret_cast<const float2*>(ep.row_stats_in) + pix * ep.stats_in_ld;
+    } else if (LINEAR) {
+        for (int c = ct; c < BLOCK_N; c += 256) s_rowvec[c] = 0.f;
+    }
+    for (int c = ct; c < BLOCK_N; c += 256)
+        s_bias[c] = (ep.bias != nullptr && col_base + c < p.N) ? __ldg(ep.bias + col_base + c) : 0.f;
+    if constexpr (LN_CONSUME) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            if (row_ok[h]) {  // fixed-order fold of the producer's per-tile partials -> mean / rstd of the row of A
+                const float2* sp = reinterpret_cast<const float2*>(ep.row_stats_in) + pix[h] * ep.stats_in_ld;
                 float s1 = 0.f, s2 = 0.f;
                 for (int i = 0; i < ep.stats_parts; ++i) {
                     const float2 t = __ldg(sp + i);
@@ -229,325 +269,212 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                     s2 += t.y;
                 }
                 const float inv = 1.0f / static_cast<float>(ep.ln_dim);
-                ln_mean = s1 * inv;
-                ln_rstd = rsqrtf(fmaxf(fmaf(-ln_mean, ln_mean, s2 * inv), 0.f) + ep.ln_eps);
+                ln_mean[h] = s1 * inv;
+                ln_rstd[h] = rsqrtf(fmaxf(fmaf(-ln_mean[h], ln_mean[h], s2 * inv), 0.f) + ep.ln_eps);
             }
         }
     }
 
     // ---- mainloop: each warpgroup multiplies its 64 rows of A by the whole B tile; the previous stage is released once
     // the MMAs that read it have retired (wait_group 1 keeps one group in flight)
-    {
-        float acc[BLOCK_N / 2];
+    float acc[BLOCK_N / 2];
 #pragma unroll
-        for (int j = 0; j < BLOCK_N / 2; ++j) acc[j] = 0.f;
-        const bool leader = (threadIdx.x & 127) == 0;
-        for (int i = 0; i < nk; ++i) {
-            const int stage = i % STAGES;
-            mbar_wait_quiet(&full_bar[stage], (i / STAGES) & 1);
-            if (i == 0 && threadIdx.x == 0) dbg_mark(p, 2);
-            const uint32_t sa = smem_u32(smem + stage * L::kStageBytes) + wg * (64 * 128);
-            const uint32_t sb = smem_u32(smem + stage * L::kStageBytes) + kABytes;
-            wgmma_fence_regs(acc);
-            wgmma_fence();
-#pragma unroll
-            for (int k = 0; k < kBlockK / 16; ++k) {
-                const uint64_t ad = wgmma_desc_sw128(sa + k * 32), bd = wgmma_desc_sw128(sb + k * 32);
-                if constexpr (BLOCK_N == 64) wgmma_m64n64k16(acc, ad, bd, 1u);
-                else if constexpr (BLOCK_N == 128) wgmma_m64n128k16(acc, ad, bd, 1u);
-                else if constexpr (BLOCK_N == 160) wgmma_m64n160k16(acc, ad, bd, 1u);
-                else wgmma_m64n256k16(acc, ad, bd, 1u);
-            }
-            wgmma_commit();
-            wgmma_wait<1>();
-            wgmma_fence_regs(acc);
-            if (i > 0 && leader) mbar_arrive(&empty_bar[(i - 1) % STAGES]);
-        }
-        wgmma_wait<0>();
+    for (int j = 0; j < BLOCK_N / 2; ++j) acc[j] = 0.f;
+    const bool leader = (threadIdx.x & 127) == 0;
+    for (int i = 0; i < nk; ++i) {
+        const int stage = i % STAGES;
+        mbar_wait_quiet(&full_bar[stage], (i / STAGES) & 1);
+        if (i == 0 && threadIdx.x == 0) dbg_mark(p, 2);
+        const uint32_t sa = smem_u32(smem + stage * L::kStageBytes) + wg * (64 * 128);
+        const uint32_t sb = smem_u32(smem + stage * L::kStageBytes) + kABytes;
         wgmma_fence_regs(acc);
-        // every MMA of the CTA has to retire before the ring is overwritten by the accumulator rows
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        if (threadIdx.x == 0) dbg_mark(p, 3);
-        if (p.pdl_late) pdl_launch_dependents();  // mainloop done: the next kernel's prologue may overlap this epilogue
-        // wgmma m64nN accumulator layout: warp w of the warpgroup holds rows 16 w + lane / 4 (+ 8), columns 8 j + 2 (lane % 4)
-        const int wrow = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+        wgmma_fence();
 #pragma unroll
-        for (int j = 0; j < BLOCK_N / 8; ++j) {
-            const int col = j * 8 + 2 * (lane & 3);
-            *reinterpret_cast<float2*>(smem + wrow * L::kAccRowBytes + col * 4) = make_float2(acc[4 * j], acc[4 * j + 1]);
-            *reinterpret_cast<float2*>(smem + (wrow + 8) * L::kAccRowBytes + col * 4) =
-                make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+        for (int k = 0; k < kBlockK / 16; ++k) {
+            const uint64_t ad = wgmma_desc_sw128(sa + k * 32), bd = wgmma_desc_sw128(sb + k * 32);
+            if constexpr (BLOCK_N == 64) wgmma_m64n64k16(acc, ad, bd, 1u);
+            else if constexpr (BLOCK_N == 128) wgmma_m64n128k16(acc, ad, bd, 1u);
+            else if constexpr (BLOCK_N == 160) wgmma_m64n160k16(acc, ad, bd, 1u);
+            else wgmma_m64n256k16(acc, ad, bd, 1u);
         }
-        asm volatile("bar.sync 1, 256;" ::: "memory");
+        wgmma_commit();
+        wgmma_wait<1>();
+        wgmma_fence_regs(acc);
+        if (i > 0 && leader) mbar_arrive(&empty_bar[(i - 1) % STAGES]);
     }
-    if (wg != 0) return;
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc);
+    if (leader) mbar_arrive(&empty_bar[(nk - 1) % STAGES]);  // the residual tile may go to this stage
+    // every MMA of the CTA has to retire before the ring is overwritten by the output tile
+    asm volatile("bar.sync 1, 256;" ::: "memory");
+    if (threadIdx.x == 0) dbg_mark(p, 3);
+    if (p.pdl_late) pdl_launch_dependents();  // mainloop done: the next kernel's prologue may overlap this epilogue
 
-    {
-        // ---------------- epilogue (warpgroup 0, thread = tile row) ----------------
-        const float alpha = ep.alpha;
-        const __nv_bfloat16* res = nullptr;
-        if (ep.residual != nullptr && row_ok)
-            res = reinterpret_cast<const __nv_bfloat16*>(ep.residual) + pix * ep.ldr;
-        const bool split = p.splits > 1;
-        uint8_t* acc_row = smem + r * L::kAccRowBytes;
-        uint4 rcur[4];
-        auto load_res = [&](int c0, uint4(&rv)[4]) {
-#pragma unroll
-            for (int g = 0; g < 4; ++g) {
-                const int cg = col_base + c0 + g * 8;
-                rv[g] = (res != nullptr && cg < p.N) ? __ldg(reinterpret_cast<const uint4*>(res + cg))
-                                                     : make_uint4(0u, 0u, 0u, 0u);
-            }
-        };
-        if (!split) load_res(0, rcur);
-        float st1 = 0.f, st2 = 0.f;  // producer: my row's statistics over this tile's columns
-        if (threadIdx.x == 0) dbg_mark(p, 4);
-
-        // ---- split-K rendezvous
+    // ---- split-K rendezvous: partials in fragment order (float4 q of consumer thread ct at [q][ct]), the last arriver
+    // sums them in split order
+    if (p.splits > 1) {
         const int64_t tile_elems = static_cast<int64_t>(kBlockM) * BLOCK_N;
         const int64_t tile_id = static_cast<int64_t>(blockIdx.y) * gridDim.x + blockIdx.x;
         const int64_t n_tiles_total = static_cast<int64_t>(gridDim.x) * gridDim.y;
-        if (split) {
-            float* mine = p.ws + (static_cast<int64_t>(blockIdx.z) * n_tiles_total + tile_id) * tile_elems +
-                          static_cast<int64_t>(r) * BLOCK_N;
-#pragma unroll 1
-            for (int c0 = 0; c0 < BLOCK_N; c0 += 4)
-                __stcg(reinterpret_cast<float4*>(mine + c0), *reinterpret_cast<const float4*>(acc_row + c0 * 4));
-            __threadfence();
-            asm volatile("bar.sync 2, 128;" ::: "memory");
-            if (threadIdx.x == 0) {
-                const unsigned int old = atomicAdd(&p.counters[tile_id], 1u);
-                *flag_slot = (old == static_cast<unsigned int>(p.splits - 1)) ? 1u : 0u;
-                if (old == static_cast<unsigned int>(p.splits - 1)) p.counters[tile_id] = 0u;  // re-arm for next launch
-            }
-            asm volatile("bar.sync 2, 128;" ::: "memory");
-            const bool last = *reinterpret_cast<volatile uint32_t*>(flag_slot) != 0u;
-            if (!last) {
-                if (threadIdx.x == 0) dbg_mark(p, 5);
-                return;
-            }
-            __threadfence();
-            load_res(0, rcur);
+        float4* mine = reinterpret_cast<float4*>(p.ws + (static_cast<int64_t>(blockIdx.z) * n_tiles_total + tile_id) * tile_elems);
+#pragma unroll
+        for (int q = 0; q < BLOCK_N / 8; ++q)
+            __stcg(mine + q * 256 + ct, make_float4(acc[4 * q], acc[4 * q + 1], acc[4 * q + 2], acc[4 * q + 3]));
+        __threadfence();
+        asm volatile("bar.sync 2, 256;" ::: "memory");
+        if (ct == 0) {
+            const unsigned int old = atomicAdd(&p.counters[tile_id], 1u);
+            *flag_slot = (old == static_cast<unsigned int>(p.splits - 1)) ? 1u : 0u;
+            if (old == static_cast<unsigned int>(p.splits - 1)) p.counters[tile_id] = 0u;  // re-arm for next launch
         }
-        // accumulator chunk loader: my staged row (single CTA per tile) or the fixed-order sum of the split partials
-        auto load_acc = [&](int c0, uint32_t(&v)[32]) {
-            if (!split) {
+        asm volatile("bar.sync 2, 256;" ::: "memory");
+        const bool last = *reinterpret_cast<volatile uint32_t*>(flag_slot) != 0u;
+        if (!last) {
+            if (ct == 0) dbg_mark(p, 5);
+            return;
+        }
+        __threadfence();
+        if (p.res_tma && ct == 0) load_residual();  // the ring is idle: no stage to wait for
 #pragma unroll
-                for (int j = 0; j < 32; j += 4) {
-                    const uint4 t = *reinterpret_cast<const uint4*>(acc_row + (c0 + j) * 4);
-                    v[j] = t.x; v[j + 1] = t.y; v[j + 2] = t.z; v[j + 3] = t.w;
-                }
-            } else {
-                float acc[32];
+        for (int j = 0; j < BLOCK_N / 2; ++j) acc[j] = 0.f;
+        for (int s = 0; s < p.splits; ++s) {
+            const float4* src = reinterpret_cast<const float4*>(p.ws + (static_cast<int64_t>(s) * n_tiles_total + tile_id) * tile_elems);
 #pragma unroll
-                for (int j = 0; j < 32; ++j) acc[j] = 0.f;
-                for (int sidx = 0; sidx < p.splits; ++sidx) {
-                    const float* src = p.ws + (static_cast<int64_t>(sidx) * n_tiles_total + tile_id) * tile_elems +
-                                       static_cast<int64_t>(r) * BLOCK_N + c0;
-#pragma unroll
-                    for (int j = 0; j < 32; j += 4) {
-                        const float4 t = __ldcg(reinterpret_cast<const float4*>(src + j));
-                        acc[j] += t.x; acc[j + 1] += t.y; acc[j + 2] += t.z; acc[j + 3] += t.w;
-                    }
-                }
-#pragma unroll
-                for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(acc[j]);
+            for (int q = 0; q < BLOCK_N / 8; ++q) {
+                const float4 t = __ldcg(src + q * 256 + ct);
+                acc[4 * q] += t.x; acc[4 * q + 1] += t.y; acc[4 * q + 2] += t.z; acc[4 * q + 3] += t.w;
             }
-        };
+        }
+    }
+    if (p.res_tma) mbar_wait_quiet(res_bar, 0);
+    if (threadIdx.x == 0) dbg_mark(p, 4);
 
-        if constexpr (LINEAR) {
-            constexpr int NCH = BLOCK_N / 32;
-            __nv_bfloat16* orow = reinterpret_cast<__nv_bfloat16*>(p.out) + pix * p.ldd + col_base;
+    // ---- epilogue from registers. Per element, in this order: alpha * acc, + bias, + row vector, activation, + residual,
+    // round. The LINEAR form always adds bias, row vector and residual (zeros when absent).
+    const float alpha = ep.alpha;
+    const bool geglu = !LINEAR && ep.act == IMAGD_ACT_GEGLU;
+    const int n_out = geglu ? p.N / 2 : p.N;
+    if (geglu) {
+        // tile = [64 value | 64 gate] columns; output columns n_blk * 64 + [0, 64): value j and gate j + 8 are both mine
+        if constexpr (BLOCK_N == 128) {
 #pragma unroll
-            for (int ch = 0; ch < NCH; ++ch) {
-                const int c0 = ch * 32;
-                uint32_t vc[32];
-                load_acc(c0, vc);
-                uint4 rnext[4];
-                if (ch + 1 < NCH) load_res(c0 + 32, rnext);
-                if (row_ok && col_base + c0 < p.N) {
+            for (int j = 0; j < 8; ++j) {
+                const int cl = 8 * j + 2 * quad;
 #pragma unroll
-                    for (int g = 0; g < 4; ++g) {
-                        const int cl = c0 + g * 8;  // tile-local column
-                        float f[8];
+                for (int h = 0; h < 2; ++h) {
+                    float o[2];
 #pragma unroll
-                        for (int j = 0; j < 8; ++j) f[j] = alpha * __uint_as_float(vc[g * 8 + j]);
-                        if constexpr (LN_CONSUME) {
-                            const float4 b0 = *reinterpret_cast<const float4*>(s_bias + cl);
-                            const float4 b1 = *reinterpret_cast<const float4*>(s_bias + cl + 4);
-                            const float4 c0v = *reinterpret_cast<const float4*>(s_rowvec + cl);
-                            const float4 c1v = *reinterpret_cast<const float4*>(s_rowvec + cl + 4);
-                            const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-                            const float cs[8] = {c0v.x, c0v.y, c0v.z, c0v.w, c1v.x, c1v.y, c1v.z, c1v.w};
-#pragma unroll
-                            for (int j = 0; j < 8; ++j) f[j] = fmaf(ln_rstd, fmaf(-ln_mean, cs[j], f[j]), bb[j]);
-                        } else {
-                            const float4 b0 = *reinterpret_cast<const float4*>(s_bias + cl);
-                            const float4 b1 = *reinterpret_cast<const float4*>(s_bias + cl + 4);
-                            f[0] += b0.x; f[1] += b0.y; f[2] += b0.z; f[3] += b0.w;
-                            f[4] += b1.x; f[5] += b1.y; f[6] += b1.z; f[7] += b1.w;
-                            const float4 r0 = *reinterpret_cast<const float4*>(s_rowvec + cl);
-                            const float4 r1 = *reinterpret_cast<const float4*>(s_rowvec + cl + 4);
-                            f[0] += r0.x; f[1] += r0.y; f[2] += r0.z; f[3] += r0.w;
-                            f[4] += r1.x; f[5] += r1.y; f[6] += r1.z; f[7] += r1.w;
+                    for (int e = 0; e < 2; ++e) {
+                        float a = alpha * acc[4 * j + 2 * h + e], g = alpha * acc[4 * (j + 8) + 2 * h + e];
+                        if constexpr (LN_CONSUME) {  // bias (folded) is mandatory here: s_bias always staged
+                            a = fmaf(ln_rstd[h], fmaf(-ln_mean[h], s_rowvec[cl + e], a), s_bias[cl + e]);
+                            g = fmaf(ln_rstd[h], fmaf(-ln_mean[h], s_rowvec[64 + cl + e], g), s_bias[64 + cl + e]);
+                        } else if (ep.bias) {
+                            a += s_bias[cl + e];
+                            g += s_bias[64 + cl + e];
                         }
-                        if (!LN_CONSUME && rowvec && col_base + cl < p.N) {  // rare: the tile spans several samples (deep levels)
-                            const float4 b0 = __ldg(reinterpret_cast<const float4*>(rowvec + col_base + cl));
-                            const float4 b1 = __ldg(reinterpret_cast<const float4*>(rowvec + col_base + cl + 4));
-                            f[0] += b0.x; f[1] += b0.y; f[2] += b0.z; f[3] += b0.w;
-                            f[4] += b1.x; f[5] += b1.y; f[6] += b1.z; f[7] += b1.w;
-                        }
-                        const uint4 rv = rcur[g];  // zeros when there is no residual
-                        f[0] += bf16lo(rv.x); f[1] += bf16hi(rv.x); f[2] += bf16lo(rv.y); f[3] += bf16hi(rv.y);
-                        f[4] += bf16lo(rv.z); f[5] += bf16hi(rv.z); f[6] += bf16lo(rv.w); f[7] += bf16hi(rv.w);
-                        const uint4 o = make_uint4(pack_bf16x2(f[0], f[1]), pack_bf16x2(f[2], f[3]),
-                                                   pack_bf16x2(f[4], f[5]), pack_bf16x2(f[6], f[7]));
-                        if constexpr (LN_PRODUCE) {  // statistics of what the consumer will READ: the rounded values
-                            if (col_base + cl < p.N) {
-                                const uint32_t ow[4] = {o.x, o.y, o.z, o.w};
-#pragma unroll
-                                for (int j = 0; j < 4; ++j) {
-                                    const float lo = bf16lo(ow[j]), hi = bf16hi(ow[j]);
-                                    st1 += lo + hi;
-                                    st2 = fmaf(lo, lo, fmaf(hi, hi, st2));
-                                }
-                            }
-                        }
-                        if constexpr (BULK) {
-                            // bytes [2 cl, 2 cl + 16) of my row: accumulator columns this thread has already read
-                            *reinterpret_cast<uint4*>(acc_row + cl * 2) = o;
-                        } else {
-                            if (col_base + cl < p.N) *reinterpret_cast<uint4*>(orow + cl) = o;
-                        }
+                        o[e] = a * gelu_erf(g);
                     }
-                }
-#pragma unroll
-                for (int g = 0; g < 4; ++g) rcur[g] = rnext[g];
-            }
-            if constexpr (BULK) {
-                // each thread ships its own row: generic-proxy writes -> async-proxy read needs the proxy fence only
-                fence_proxy_async_smem();
-                const int valid = min(BLOCK_N, p.N - col_base);
-                if (row_ok && valid > 0) bulk_store_s2g(orow, smem_u32(acc_row), static_cast<uint32_t>(valid) * 2u);
-                bulk_commit();
-                bulk_wait_read0();  // the staging bytes must stay valid until the copy engine has read them
-            }
-            if constexpr (LN_PRODUCE) {
-                if (row_ok)
-                    reinterpret_cast<float2*>(ep.row_stats_out)[pix * ep.stats_ld + n_blk] = make_float2(st1, st2);
-            }
-        } else if (ep.act == IMAGD_ACT_GEGLU) {
-            // tile = [64 value | 64 gate]; output columns n_blk*64 + [0, 64)
-            if constexpr (BLOCK_N == 128) {
-#pragma unroll 1
-                for (int c0 = 0; c0 < 64; c0 += 32) {
-                    uint32_t va[32], vg[32];
-                    load_acc(c0, va);
-                    load_acc(64 + c0, vg);
-                    const int pcol = n_blk * 128 + c0;  // packed column of value; gate at +64
-                    const int ocol = n_blk * 64 + c0;
-                    if (row_ok && pcol < p.N) {
-                        uint32_t packed[16];
-#pragma unroll
-                        for (int j = 0; j < 32; j += 2) {
-                            float a0 = alpha * __uint_as_float(va[j]), a1 = alpha * __uint_as_float(va[j + 1]);
-                            float g0 = alpha * __uint_as_float(vg[j]), g1 = alpha * __uint_as_float(vg[j + 1]);
-                            if constexpr (LN_CONSUME) {  // bias (folded) is mandatory here: s_bias always staged
-                                const float2 ba = *reinterpret_cast<const float2*>(s_bias + c0 + j);
-                                const float2 bg = *reinterpret_cast<const float2*>(s_bias + 64 + c0 + j);
-                                const float2 ca = *reinterpret_cast<const float2*>(s_rowvec + c0 + j);
-                                const float2 cg = *reinterpret_cast<const float2*>(s_rowvec + 64 + c0 + j);
-                                a0 = fmaf(ln_rstd, fmaf(-ln_mean, ca.x, a0), ba.x);
-                                a1 = fmaf(ln_rstd, fmaf(-ln_mean, ca.y, a1), ba.y);
-                                g0 = fmaf(ln_rstd, fmaf(-ln_mean, cg.x, g0), bg.x);
-                                g1 = fmaf(ln_rstd, fmaf(-ln_mean, cg.y, g1), bg.y);
-                            } else if (ep.bias) {
-                                const float2 ba = *reinterpret_cast<const float2*>(s_bias + c0 + j);
-                                const float2 bg = *reinterpret_cast<const float2*>(s_bias + 64 + c0 + j);
-                                a0 += ba.x;
-                                a1 += ba.y;
-                                g0 += bg.x;
-                                g1 += bg.y;
-                            }
-                            packed[j / 2] = pack_bf16x2(a0 * gelu_erf(g0), a1 * gelu_erf(g1));
-                        }
-                        uint4* dst = reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(p.out) + pix * p.ldd + ocol);
-#pragma unroll
-                        for (int q = 0; q < 4; ++q)
-                            dst[q] = make_uint4(packed[4 * q], packed[4 * q + 1], packed[4 * q + 2], packed[4 * q + 3]);
-                    }
+                    const int r = frow + 8 * h;
+                    *reinterpret_cast<uint32_t*>(epi_chunk(cl / kEpiCols) + epi_offset(r, cl % kEpiCols)) =
+                        pack_bf16x2(o[0], o[1]);
                 }
             }
-        } else {
-#pragma unroll 1
-            for (int c0 = 0; c0 < BLOCK_N; c0 += 32) {
-                uint32_t v[32];
-                load_acc(c0, v);
-                uint4 rnext[4];
-                if (c0 + 32 < BLOCK_N) load_res(c0 + 32, rnext);  // in flight while this chunk is processed
-                const int col = col_base + c0;
-                if (row_ok && col < p.N) {
-                // row vector fallback (tile spans several samples): all of the chunk's loads issued together
-                float4 rvv[8];
-                if (rowvec) {
+        }
+    } else {
+        const bool add_bias = LINEAR || ep.bias != nullptr;
+        const bool add_rowvec = LINEAR || ep.rowvec != nullptr;
+        const bool add_res = LINEAR || p.res_tma;
+        const int act = LINEAR ? IMAGD_ACT_NONE : ep.act;
+        float st1[2] = {0.f, 0.f}, st2[2] = {0.f, 0.f};  // LayerNorm producer: my rows' statistics over this tile
 #pragma unroll
-                    for (int q = 0; q < 8; ++q)
-                        rvv[q] = (col + q * 4 < p.N) ? __ldg(reinterpret_cast<const float4*>(rowvec + col + q * 4))
-                                                     : make_float4(0.f, 0.f, 0.f, 0.f);
-                }
-                // columns are handled in groups of 8 (N % 8 == 0 is enforced on the host)
+        for (int j = 0; j < BLOCK_N / 8; ++j) {
+            const int cl = 8 * j + 2 * quad;  // tile-local column of element e = 0
+            const bool col_ok = col_base + cl < p.N;  // (N % 8 == 0: both elements or neither)
+            uint8_t* chunk = epi_chunk(cl / kEpiCols);
 #pragma unroll
-                for (int g = 0; g < 4; ++g) {
-                    const int cg = col + g * 8;
-                    if (cg >= p.N) break;
-                    float f[8];
+            for (int h = 0; h < 2; ++h) {
+                const int r = frow + 8 * h;
+                float f[2];
 #pragma unroll
-                    for (int j = 0; j < 8; ++j) f[j] = alpha * __uint_as_float(v[g * 8 + j]);
-                    if (ep.bias) {
-                        const float4 b0 = *reinterpret_cast<const float4*>(s_bias + c0 + g * 8);
-                        const float4 b1 = *reinterpret_cast<const float4*>(s_bias + c0 + g * 8 + 4);
-                        f[0] += b0.x; f[1] += b0.y; f[2] += b0.z; f[3] += b0.w;
-                        f[4] += b1.x; f[5] += b1.y; f[6] += b1.z; f[7] += b1.w;
+                for (int e = 0; e < 2; ++e) f[e] = alpha * acc[4 * j + 2 * h + e];
+                if constexpr (LN_CONSUME) {
+#pragma unroll
+                    for (int e = 0; e < 2; ++e)
+                        f[e] = fmaf(ln_rstd[h], fmaf(-ln_mean[h], s_rowvec[cl + e], f[e]), s_bias[cl + e]);
+                } else {
+                    if (add_bias) {
+                        f[0] += s_bias[cl];
+                        f[1] += s_bias[cl + 1];
                     }
-                    if (rowvec_shared) {
-                        const float4 b0 = *reinterpret_cast<const float4*>(s_rowvec + c0 + g * 8);
-                        const float4 b1 = *reinterpret_cast<const float4*>(s_rowvec + c0 + g * 8 + 4);
-                        f[0] += b0.x; f[1] += b0.y; f[2] += b0.z; f[3] += b0.w;
-                        f[4] += b1.x; f[5] += b1.y; f[6] += b1.z; f[7] += b1.w;
-                    } else if (rowvec) {
-                        const float4 b0 = rvv[2 * g], b1 = rvv[2 * g + 1];
-                        f[0] += b0.x; f[1] += b0.y; f[2] += b0.z; f[3] += b0.w;
-                        f[4] += b1.x; f[5] += b1.y; f[6] += b1.z; f[7] += b1.w;
-                    }
-                    if (ep.act == IMAGD_ACT_SILU) {
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) f[j] = silu(f[j]);
-                    } else if (ep.act == IMAGD_ACT_GELU) {
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) f[j] = gelu_erf(f[j]);
-                    } else if (ep.act == IMAGD_ACT_QUICK_GELU) {  // x * sigmoid(1.702 x): CLIP text MLP (quick_gelu)
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) f[j] = __fdividef(f[j], 1.0f + __expf(-1.702f * f[j]));
-                    }
-                    if (res) {
-                        const uint4 rv = rcur[g];
-                        f[0] += bf16lo(rv.x); f[1] += bf16hi(rv.x); f[2] += bf16lo(rv.y); f[3] += bf16hi(rv.y);
-                        f[4] += bf16lo(rv.z); f[5] += bf16hi(rv.z); f[6] += bf16lo(rv.w); f[7] += bf16hi(rv.w);
-                    }
-                    if (ep.out_fp32) {
-                        float4* dst = reinterpret_cast<float4*>(reinterpret_cast<float*>(p.out) + pix * p.ldd + cg);
-                        dst[0] = make_float4(f[0], f[1], f[2], f[3]);
-                        dst[1] = make_float4(f[4], f[5], f[6], f[7]);
-                    } else {
-                        uint4* dst = reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(p.out) + pix * p.ldd + cg);
-                        *dst = make_uint4(pack_bf16x2(f[0], f[1]), pack_bf16x2(f[2], f[3]), pack_bf16x2(f[4], f[5]),
-                                          pack_bf16x2(f[6], f[7]));
+                    if (add_rowvec) {
+                        const float2 v = col_ok ? *reinterpret_cast<const float2*>(rowvec[h] + cl) : make_float2(0.f, 0.f);
+                        f[0] += v.x;
+                        f[1] += v.y;
                     }
                 }
+                if (act == IMAGD_ACT_SILU) {
+                    f[0] = silu(f[0]);
+                    f[1] = silu(f[1]);
+                } else if (act == IMAGD_ACT_GELU) {
+                    f[0] = gelu_erf(f[0]);
+                    f[1] = gelu_erf(f[1]);
+                } else if (act == IMAGD_ACT_QUICK_GELU) {  // x * sigmoid(1.702 x): CLIP text MLP (quick_gelu)
+                    f[0] = __fdividef(f[0], 1.0f + __expf(-1.702f * f[0]));
+                    f[1] = __fdividef(f[1], 1.0f + __expf(-1.702f * f[1]));
                 }
-#pragma unroll
-                for (int g = 0; g < 4; ++g) rcur[g] = rnext[g];
+                uint32_t* slot = reinterpret_cast<uint32_t*>(chunk + epi_offset(r, cl % kEpiCols));
+                if (add_res) {  // the residual tile is staged where the output goes (zeros beyond N)
+                    const uint32_t rv = p.res_tma ? *slot : 0u;
+                    f[0] += bf16lo(rv);
+                    f[1] += bf16hi(rv);
+                }
+                if (!LINEAR && ep.out_fp32) {
+                    if (row_ok[h] && col_ok)
+                        *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + pix[h] * p.ldd + col_base + cl) =
+                            make_float2(f[0], f[1]);
+                    continue;
+                }
+                const uint32_t o = pack_bf16x2(f[0], f[1]);
+                if constexpr (LN_PRODUCE) {  // statistics of what the consumer will READ: the rounded values
+                    if (col_ok) {
+                        const float lo = bf16lo(o), hi = bf16hi(o);
+                        st1[h] += lo + hi;
+                        st2[h] = fmaf(lo, lo, fmaf(hi, hi, st2[h]));
+                    }
+                }
+                if constexpr (UPS) {
+                    if (row_ok[h] && col_ok)
+                        *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.out) + pix[h] * p.ldd + col_base + cl) = o;
+                } else {
+                    *slot = o;
+                }
             }
+        }
+        if constexpr (LN_PRODUCE) {  // the quad holds the row's columns: reduce, one write per row and N tile
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+#pragma unroll
+                for (int m = 1; m < 4; m <<= 1) {
+                    st1[h] += __shfl_xor_sync(0xffffffffu, st1[h], m);
+                    st2[h] += __shfl_xor_sync(0xffffffffu, st2[h], m);
+                }
+                int64_t px;  // (recomputed: keeping the pixel index live through the loop costs registers at BLOCK_N 256)
+                if (quad == 0 && row_at(h, px))
+                    reinterpret_cast<float2*>(ep.row_stats_out)[px * ep.stats_ld + n_blk] = make_float2(st1[h], st2[h]);
+            }
+        }
+    }
+    if (p.store_tma) {
+        fence_proxy_async_smem();  // generic-proxy writes -> async-proxy reads
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+        if (ct == 0) {
+            const int oc0 = geglu ? n_blk * 64 : col_base;
+            const int chunks = geglu ? 64 / kEpiCols : BLOCK_N / kEpiCols;
+            for (int c = 0; c < chunks && oc0 + c * kEpiCols < n_out; ++c)
+                tma_store_4d(&tmD, epi_chunk(c), oc0 + c * kEpiCols, x0, y0, n0);
+            bulk_commit();
+            bulk_wait_read0();  // the staged tile must stay valid until the copy engine has read it
         }
     }
     if (threadIdx.x == 0) dbg_mark(p, 5);
@@ -612,8 +539,8 @@ static int ensure_scratch(float** ws, unsigned int** counters, cudaStream_t stre
 
 // ---- tile / pipeline-depth / split-K choice --------------------------------------------------------------------
 // Variants: N tile 64 / 128 / 160 / 256 with a "shallow" (2-4 stages) or "deep" (4-8 stages, ~190 KB) operand ring. Every
-// variant runs one CTA per SM (the register file allows no second one); the shared-memory footprint is max(ring,
-// 128 x (4 BN + 16) bytes of accumulator staging) plus the epilogue vectors (about 96-200 KB).
+// variant runs one CTA per SM (the register file allows no second one); the shared-memory footprint is the ring plus the
+// epilogue vectors (about 96-200 KB): the residual / output tiles of the epilogue reuse the ring.
 //
 // Measured on an H100 80GB HBM3 (SXM, 400 W power limit, 1980 MHz max SM clock) with tools/gemm_bench.py over the 92
 // launch keys of a denoising step at batch 1 and 8, every variant timed in isolation:
@@ -625,7 +552,8 @@ static int ensure_scratch(float** ws, unsigned int** counters, cudaStream_t stre
 // So the rule minimises  waves x (t_wave(BN) + k-blocks per CTA x t_kb(BN)) + t_split x (MB of split-K partials)  with
 // waves = ceil(CTAs / 132), t_kb / t_wave (prologue + epilogue) fitted by least squares to those timings. With it the
 // step's GEMM + conv launches take 4.6 ms instead of 6.2 ms at batch 1 and 28.4 ms instead of 32.7 ms at batch 8
-// (sum of the isolated launch times, same card).
+// (sum of the isolated launch times, same card). The constants were fitted with the earlier epilogue, which staged the
+// fp32 accumulator tile through shared memory; the register epilogue lowers t_wave, and they have not been re-fitted.
 struct GemmCfg {
     int bn, stages, splits;
 };
@@ -662,46 +590,36 @@ static GemmCfg choose_cfg(int m_tiles, int N, int kb_total, bool geglu, bool all
     return best;
 }
 
-template <int BLOCK_N, int STAGES, int EPI, int LNM = 0>
-static int launch_gemm_impl(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, int m_tiles,
-                            cudaStream_t stream) {
+template <int BLOCK_N, int STAGES, bool LINEAR, int LNM = 0>
+static int launch_gemm_impl(const CUtensorMap (&tm)[4], const GemmParams& p, int m_tiles, cudaStream_t stream) {
     using L = GemmSmem<BLOCK_N, STAGES>;
     constexpr int kSmem = L::kTotal;
-    IMAGD_SET_MAX_SMEM((gemm_tc_kernel<BLOCK_N, STAGES, EPI, LNM>), kSmem);
+    IMAGD_SET_MAX_SMEM((gemm_tc_kernel<BLOCK_N, STAGES, LINEAR, LNM>), kSmem);
     const int n_tiles = (p.N + BLOCK_N - 1) / BLOCK_N;
     dim3 grid(m_tiles, LNM == 3 ? 4 * n_tiles : n_tiles, p.splits);
-    IMAGD_CUDA(launch_pdl(gemm_tc_kernel<BLOCK_N, STAGES, EPI, LNM>, grid, dim3(kGemmThreads), kSmem, stream, tmA, tmB, p));
+    IMAGD_CUDA(launch_pdl(gemm_tc_kernel<BLOCK_N, STAGES, LINEAR, LNM>, grid, dim3(kGemmThreads), kSmem, stream, tm[0], tm[1],
+                          tm[2], tm[3], p));
     return IMAGD_OK;
 }
 
+// tm = {A, B, residual, output}
 template <int BLOCK_N, int STAGES>
-static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, int m_tiles,
-                       cudaStream_t stream) {
+static int launch_gemm(const CUtensorMap (&tm)[4], const GemmParams& p, int m_tiles, cudaStream_t stream) {
     const bool linear = p.ep.act == IMAGD_ACT_NONE && !p.ep.out_fp32;
     if (p.ups_n_tiles > 0) {  // upsample-phase conv: plain bf16 epilogue (bias only), validated by the caller
         GemmParams q = p;
         q.ups_n_tiles = (p.N + BLOCK_N - 1) / BLOCK_N;
-        return launch_gemm_impl<BLOCK_N, STAGES, 1, 3>(tmA, tmB, q, m_tiles, stream);
+        return launch_gemm_impl<BLOCK_N, STAGES, true, 3>(tm, q, m_tiles, stream);
     }
-    // LayerNorm folding variants (plain stores only for now; the bulk-store combination comes after validation)
-    if (p.ep.row_stats_out != nullptr) return launch_gemm_impl<BLOCK_N, STAGES, 1, 1>(tmA, tmB, p, m_tiles, stream);
+    if (p.ep.row_stats_out != nullptr) return launch_gemm_impl<BLOCK_N, STAGES, true, 1>(tm, p, m_tiles, stream);
     if (p.ep.row_stats_in != nullptr) {
-        if (linear) return launch_gemm_impl<BLOCK_N, STAGES, 1, 2>(tmA, tmB, p, m_tiles, stream);
-        if constexpr (BLOCK_N == 128) return launch_gemm_impl<BLOCK_N, STAGES, 0, 2>(tmA, tmB, p, m_tiles, stream);
+        if (linear) return launch_gemm_impl<BLOCK_N, STAGES, true, 2>(tm, p, m_tiles, stream);
+        if constexpr (BLOCK_N == 128) return launch_gemm_impl<BLOCK_N, STAGES, false, 2>(tm, p, m_tiles, stream);
         set_error("gemm: LayerNorm-folded generic epilogue exists for the GEGLU tile (128) only");
         return IMAGD_ERR_ARG;
     }
-    // Bulk row stores: for grids that cover the chip more than twice. IMAGD_GEMM_BULK_STORE = 0 / 1 forces them off / on.
-    static int bulk_env = -2;
-    if (bulk_env == -2) {
-        const char* e = getenv("IMAGD_GEMM_BULK_STORE");
-        bulk_env = e ? (e[0] == '1' ? 1 : 0) : -1;
-    }
-    const int64_t ctas = static_cast<int64_t>(m_tiles) * ((p.N + BLOCK_N - 1) / BLOCK_N) * p.splits;
-    const bool bulk = bulk_env >= 0 ? bulk_env == 1 : ctas > 2 * kNumSms;
-    if (!linear) return launch_gemm_impl<BLOCK_N, STAGES, 0>(tmA, tmB, p, m_tiles, stream);
-    if (!bulk) return launch_gemm_impl<BLOCK_N, STAGES, 1>(tmA, tmB, p, m_tiles, stream);
-    return launch_gemm_impl<BLOCK_N, STAGES, 2>(tmA, tmB, p, m_tiles, stream);
+    if (linear) return launch_gemm_impl<BLOCK_N, STAGES, true>(tm, p, m_tiles, stream);
+    return launch_gemm_impl<BLOCK_N, STAGES, false>(tm, p, m_tiles, stream);
 }
 
 
@@ -802,32 +720,53 @@ static int run_gemm_like(const void* A, int64_t lda, int NB, int H, int W, int C
     }
 
     // A: [NB, H, W, lda] viewed (c, x, y, n)
-    CUtensorMap tmA, tmB;
+    CUtensorMap tm[4];  // A, B, residual, output
     {
         uint64_t dims[4] = {static_cast<uint64_t>(Cin), static_cast<uint64_t>(W), static_cast<uint64_t>(H),
                             static_cast<uint64_t>(NB)};
         uint64_t strides[3] = {static_cast<uint64_t>(lda) * 2, static_cast<uint64_t>(lda) * 2 * W,
                                static_cast<uint64_t>(lda) * 2 * W * H};
         uint32_t box[4] = {kBlockK, static_cast<uint32_t>(p.bw), static_cast<uint32_t>(p.bh), static_cast<uint32_t>(p.bn)};
-        int rc = make_tmap_bf16(&tmA, A, 4, dims, strides, box);
+        int rc = make_tmap_bf16(&tm[0], A, 4, dims, strides, box);
         if (rc != IMAGD_OK) return rc;
     }
     {
         uint64_t dims[2] = {static_cast<uint64_t>(taps) * Cin, static_cast<uint64_t>(N) * (ups_mode ? 4 : 1)};
         uint64_t strides[1] = {static_cast<uint64_t>(ldw) * 2};
         uint32_t box[2] = {kBlockK, static_cast<uint32_t>(cfg.bn)};
-        int rc = make_tmap_bf16(&tmB, Wt, 2, dims, strides, box);
+        int rc = make_tmap_bf16(&tm[1], Wt, 2, dims, strides, box);
+        if (rc != IMAGD_OK) return rc;
+    }
+    // residual and output: the same (c, x, y, n) pixel geometry with the logical column count, in 32-column boxes; the
+    // extents clip ragged tiles, so a launch writing a column slice of a wider buffer leaves the other columns alone
+    auto pixel_map = [&](CUtensorMap* m, const void* base, int64_t ld, int cols) {
+        uint64_t dims[4] = {static_cast<uint64_t>(cols), static_cast<uint64_t>(W), static_cast<uint64_t>(H),
+                            static_cast<uint64_t>(NB)};
+        uint64_t strides[3] = {static_cast<uint64_t>(ld) * 2, static_cast<uint64_t>(ld) * 2 * W,
+                               static_cast<uint64_t>(ld) * 2 * W * H};
+        uint32_t box[4] = {kEpiCols, static_cast<uint32_t>(p.bw), static_cast<uint32_t>(p.bh), static_cast<uint32_t>(p.bn)};
+        return make_tmap_bf16(m, base, 4, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_64B);
+    };
+    p.res_tma = ep.residual != nullptr && !geglu;
+    p.store_tma = !ep.out_fp32 && !ups_mode;
+    tm[2] = tm[3] = tm[0];
+    if (p.res_tma) {
+        int rc = pixel_map(&tm[2], ep.residual, ep.ldr, N);
+        if (rc != IMAGD_OK) return rc;
+    }
+    if (p.store_tma) {
+        int rc = pixel_map(&tm[3], D, ldd, geglu ? N / 2 : N);
         if (rc != IMAGD_OK) return rc;
     }
     switch (cfg.bn * 100 + cfg.stages) {
-        case 6404: return launch_gemm<64, 4>(tmA, tmB, p, m_tiles, stream);
-        case 6408: return launch_gemm<64, 8>(tmA, tmB, p, m_tiles, stream);
-        case 12803: return launch_gemm<128, 3>(tmA, tmB, p, m_tiles, stream);
-        case 12806: return launch_gemm<128, 6>(tmA, tmB, p, m_tiles, stream);
-        case 16003: return launch_gemm<160, 3>(tmA, tmB, p, m_tiles, stream);
-        case 16005: return launch_gemm<160, 5>(tmA, tmB, p, m_tiles, stream);
-        case 25602: return launch_gemm<256, 2>(tmA, tmB, p, m_tiles, stream);
-        case 25604: return launch_gemm<256, 4>(tmA, tmB, p, m_tiles, stream);
+        case 6404: return launch_gemm<64, 4>(tm, p, m_tiles, stream);
+        case 6408: return launch_gemm<64, 8>(tm, p, m_tiles, stream);
+        case 12803: return launch_gemm<128, 3>(tm, p, m_tiles, stream);
+        case 12806: return launch_gemm<128, 6>(tm, p, m_tiles, stream);
+        case 16003: return launch_gemm<160, 3>(tm, p, m_tiles, stream);
+        case 16005: return launch_gemm<160, 5>(tm, p, m_tiles, stream);
+        case 25602: return launch_gemm<256, 2>(tm, p, m_tiles, stream);
+        case 25604: return launch_gemm<256, 4>(tm, p, m_tiles, stream);
         default:
             set_error("gemm: no kernel variant for N tile %d with %d stages", cfg.bn, cfg.stages);
             return IMAGD_ERR_ARG;

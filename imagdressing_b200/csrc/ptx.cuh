@@ -113,6 +113,14 @@ __device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* m
         "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
         : "memory");
 }
+// Tile store shared -> global through the tensor map (out-of-bounds elements of the box are not written), tracked by the
+// issuing thread's bulk group (bulk_commit / bulk_wait_read0). Shared-memory writes of other threads need
+// fence_proxy_async_smem and a barrier first.
+__device__ __forceinline__ void tma_store_4d(const CUtensorMap* m, const void* smem_src, int c0, int c1, int c2, int c3) {
+    asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
+                 ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+                 : "memory");
+}
 
 // ---------------------------------------------------------------- wgmma (warpgroup MMA, sm_90a)
 // Shared-memory matrix descriptor for a K-major operand in the 128-byte swizzle TMA writes (rows of 64 bf16 = 128 B,
