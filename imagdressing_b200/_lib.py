@@ -81,6 +81,10 @@ SIGNATURES = {
     "imagd_attention_causal_bf16": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_int, c_int, c_int, c_int,
                                             POINTER(KVStream), c_float, c_void_p]),
     "imagd_groupnorm_ws_bytes": (c_int64, [c_int, c_int, c_int, c_int]),
+    "imagd_groupnorm_plan": (c_int, [c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "imagd_groupnorm_cluster_capacity": (c_int, [c_void_p]),
+    "imagd_groupnorm_debug_force": (c_int, [c_int, c_int, c_int]),
+    "imagd_groupnorm_debug_log": (c_int, [c_int, c_char_p, c_int]),
     "imagd_groupnorm_bf16": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_void_p,
                                      c_void_p, c_float, c_int, c_void_p, c_void_p]),
     "imagd_layernorm_bf16": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p, c_float,

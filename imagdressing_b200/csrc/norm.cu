@@ -2,7 +2,13 @@
 // 128-bit loads, statistics are fp32 with fixed-order (bit-reproducible) reductions.
 #include <cooperative_groups.h>
 
-#include <cstdlib>
+#include <algorithm>
+#include <cstdio>
+#include <cstring>
+#include <mutex>
+#include <string>
+#include <utility>
+#include <vector>
 
 #include "common.cuh"
 #include "ptx.cuh"
@@ -13,32 +19,13 @@ constexpr int kGnMaxC = 2560;
 constexpr int kGnThreads = 512;
 constexpr int kGnCounters = 1024;  // max samples per call
 
-// Chunks (CTAs) per sample. Every CTA of the launch must be resident at once (the kernel contains a sample-wide
-// rendezvous), so the grid is capped at 2 CTAs per SM — the occupancy __launch_bounds__(512, 2) guarantees.
-// Tuning knob IMAGD_GN_PX (default 16: B=1 step 6.14 -> 6.00 ms vs 32, B=8 neutral): smaller = more, shorter CTAs.
-static int gn_pixels_per_chunk() {
-    static int v = 0;
-    if (v == 0) {
-        const char* e = getenv("IMAGD_GN_PX");
-        v = e ? atoi(e) : 16;
-        if (v < 4 || v > 256) v = 16;
-    }
-    return v;
-}
-static int gn_max_chunks() {  // IMAGD_GN_MAXCHUNKS, default 64
-    static int v = 0;
-    if (v == 0) {
-        const char* e = getenv("IMAGD_GN_MAXCHUNKS");
-        v = e ? atoi(e) : 64;
-        if (v < 1 || v > kNumSms) v = 64;
-    }
-    return v;
-}
+// Chunks (CTAs) per sample of the rendezvous kernel: at least 16 pixels each, at most 64 per sample. Every CTA of the
+// launch must be resident at once (the kernel contains a sample-wide rendezvous), so the grid is capped at 2 CTAs per
+// SM — the occupancy __launch_bounds__(512, 2) guarantees.
 inline int gn_chunks(int HW, int NB) {
-    const int px = gn_pixels_per_chunk();
-    int c = (HW + px - 1) / px;
+    int c = (HW + 15) / 16;
     const int cap = (kNumSms * 2) / (NB > 0 ? NB : 1);
-    if (c > gn_max_chunks()) c = gn_max_chunks();
+    if (c > 64) c = 64;
     if (c > cap) c = cap;
     return c < 1 ? 1 : c;
 }
@@ -274,13 +261,15 @@ __global__ void __launch_bounds__(kGnThreads, 2) groupnorm_fused_kernel(
     }
 }
 
-// Cluster GroupNorm for the latency-bound regime (batch 1: a handful of CTAs per sample, where the L2 rendezvous of the
-// kernel above costs more than the data movement). A cluster of kGnCS CTAs owns one (sample, slice of whole groups):
+// Cluster GroupNorm: the kernel of the launches whose clusters are all co-resident (gn_plan: everything below level 0
+// of the UNet step at batch 1, the two inner levels at batch 8). A cluster of CS CTAs owns one (sample, slice of whole groups):
 // CTA r keeps rows [r * rpc, (r + 1) * rpc) x the slice's channels IN SHARED MEMORY, so every element is read from
 // global memory exactly once; the per-CTA {mean, M2} partials are exchanged through distributed shared memory between
 // two cluster barriers (no L2 atomics, no co-residency assumption, clusters are independent), merged by every CTA in
 // rank order (bit-reproducible, same shifted / Chan arithmetic as above), and the tile is normalised out of shared memory.
-constexpr int kGnCS = 8;  // portable cluster size
+// Every CTA reaches both cluster barriers on every path: a CTA whose row range is empty (HW < CS * rpc) contributes a
+// zero-count partial and normalises nothing, it never returns early.
+template <int CS>
 __global__ void __launch_bounds__(kGnThreads, 2) groupnorm_cluster_kernel(
     const __nv_bfloat16* __restrict__ x, int64_t ldx, __nv_bfloat16* __restrict__ y, int64_t ldy, int HW, int C,
     int groups, int gps, const float* __restrict__ gamma, const float* __restrict__ beta, float eps, int fuse_silu,
@@ -291,7 +280,7 @@ __global__ void __launch_bounds__(kGnThreads, 2) groupnorm_cluster_kernel(
     cg::cluster_group cluster = cg::this_cluster();
     __shared__ float s_a[kGnThreads * 8];  // phase 1: per (row slot, channel) sums      | phase 2: per-channel scale
     __shared__ float s_b[kGnThreads * 8];  // phase 1: per (row slot, channel) sum of sq | phase 2: per-channel shift
-    __shared__ float s_part[64 * 2];       // my {mean, M2} per group of the slice: what the other CTAs of the cluster read
+    __shared__ __align__(8) float s_part[64 * 2];  // my {mean, M2} per group of the slice: what the other CTAs of the cluster read
     __shared__ float s_mean[64];
     __shared__ float s_rstd[64];
     extern __shared__ __align__(16) unsigned char s_dyn[];
@@ -303,9 +292,9 @@ __global__ void __launch_bounds__(kGnThreads, 2) groupnorm_cluster_kernel(
     float* s_piv = s_beta + SC;
     uint4* tile = reinterpret_cast<uint4*>(s_dyn + ((3 * SC * sizeof(float) + 15) / 16) * 16);
     const int rank = static_cast<int>(cluster.block_rank());
-    const int slice = blockIdx.x / kGnCS, n = blockIdx.y;
+    const int slice = blockIdx.x / CS, n = blockIdx.y;
     const int c_base = slice * SC;
-    const int rpc = (HW + kGnCS - 1) / kGnCS;
+    const int rpc = (HW + CS - 1) / CS;
     const int p_begin = min(HW, rank * rpc);
     const int p_end = min(HW, p_begin + rpc);
     for (int c = threadIdx.x; c < SC; c += kGnThreads) {
@@ -336,23 +325,20 @@ __global__ void __launch_bounds__(kGnThreads, 2) groupnorm_cluster_kernel(
         }
         for (int pix = p_begin + prow; pix < p_end; pix += rows * 4) {
             uint4 v[4];
-            float live[4];
 #pragma unroll
             for (int t = 0; t < 4; ++t) {
                 v[t] = make_uint4(0u, 0u, 0u, 0u);
-                live[t] = 0.f;
-                if (pix + t * rows < p_end) {
+                if (pix + t * rows < p_end)
                     v[t] = __ldg(reinterpret_cast<const uint4*>(base + static_cast<int64_t>(pix + t * rows) * ldx));
-                    live[t] = 1.f;
-                }
             }
 #pragma unroll
             for (int t = 0; t < 4; ++t) {
-                if (pix + t * rows < p_end) tile[(pix + t * rows - p_begin) * SV + cv] = v[t];
+                if (pix + t * rows >= p_end) break;  // a masked-out pixel contributes nothing
+                tile[(pix + t * rows - p_begin) * SV + cv] = v[t];
                 const uint32_t u[4] = {v[t].x, v[t].y, v[t].z, v[t].w};
 #pragma unroll
                 for (int k = 0; k < 4; ++k) {
-                    const float a = (bf16lo(u[k]) - piv[2 * k]) * live[t], b = (bf16hi(u[k]) - piv[2 * k + 1]) * live[t];
+                    const float a = bf16lo(u[k]) - piv[2 * k], b = bf16hi(u[k]) - piv[2 * k + 1];
                     sum[2 * k] += a;
                     sq[2 * k] += a * a;
                     sum[2 * k + 1] += b;
@@ -367,11 +353,26 @@ __global__ void __launch_bounds__(kGnThreads, 2) groupnorm_cluster_kernel(
         }
     }
     __syncthreads();
-    for (int c = threadIdx.x; c < SC; c += kGnThreads) {  // fold the row slots (fixed order)
-        float a = s_a[c], b = s_b[c];
-        for (int r = 1; r < rows; ++r) {
+    // fold the row slots in two fixed-order stages (a narrow slice has ~100 slots: one thread per channel walking all of
+    // them is a serial chain of shared-memory loads): slot p of `parts` first takes slots p, p + parts, ... in place
+    // (nobody else reads slot p), then the channel's thread adds the `parts` survivors
+    const int parts = max(1, min(rows, kGnThreads / SC));
+    for (int idx = threadIdx.x; idx < SC * parts; idx += kGnThreads) {
+        const int c = idx % SC, p = idx / SC;
+        float a = s_a[p * SC + c], b = s_b[p * SC + c];
+        for (int r = p + parts; r < rows; r += parts) {
             a += s_a[r * SC + c];
             b += s_b[r * SC + c];
+        }
+        s_a[p * SC + c] = a;
+        s_b[p * SC + c] = b;
+    }
+    __syncthreads();
+    for (int c = threadIdx.x; c < SC; c += kGnThreads) {
+        float a = s_a[c], b = s_b[c];
+        for (int p = 1; p < parts; ++p) {
+            a += s_a[p * SC + c];
+            b += s_b[p * SC + c];
         }
         s_a[c] = a;
         s_b[c] = b;
@@ -396,13 +397,16 @@ __global__ void __launch_bounds__(kGnThreads, 2) groupnorm_cluster_kernel(
     if (threadIdx.x < gps) {  // CTAs -> sample, in rank order, relative to rank 0's mean
         const int g = threadIdx.x;
         float a = 0.f, b = 0.f;
-        const float pivot = cluster.map_shared_rank(s_part, 0)[2 * g];
-        for (int r = 0; r < kGnCS; ++r) {
-            const float* rp = cluster.map_shared_rank(s_part, r);
+        float2 part[CS];  // all remote reads in flight together
+#pragma unroll
+        for (int r = 0; r < CS; ++r) part[r] = reinterpret_cast<const float2*>(cluster.map_shared_rank(s_part, r))[g];
+        const float pivot = part[0].x;
+#pragma unroll
+        for (int r = 0; r < CS; ++r) {
             const float cnt_r = static_cast<float>(cpg) * static_cast<float>(max(min(HW, (r + 1) * rpc) - min(HW, r * rpc), 0));
-            const float d = rp[2 * g] - pivot;
+            const float d = part[r].x - pivot;
             a += cnt_r * d;
-            b += rp[2 * g + 1] + cnt_r * d * d;
+            b += part[r].y + cnt_r * d * d;
         }
         const float cnt = static_cast<float>(cpg) * static_cast<float>(HW);
         const float dm = a / cnt;
@@ -542,55 +546,136 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const __nv_bfloat16* __r
     }
 }
 
-// Which GroupNorm kernel: IMAGD_GN_CLUSTER = 0 the chunked rendezvous kernel always; 1 (default) the cluster kernel in the
-// latency-bound regime it exists for — the whole launch is one wave of clusters and a CTA's tile is at most 32 KB; 2 whenever
-// a slice fits shared memory. Large tiles stay on the rendezvous kernel, whose shorter CTAs spread them over more SMs.
-static int gn_cluster_mode() {
-    static int v = -1;
-    if (v < 0) {
-        const char* e = getenv("IMAGD_GN_CLUSTER");
-        v = e ? atoi(e) : 1;
-        if (v < 0 || v > 2) v = 1;
-    }
-    return v;
-}
-struct GnClusterPlan {
-    int gps;      // groups per slice
-    size_t smem;  // dynamic shared memory per CTA
+// ---- which GroupNorm kernel, and how the cluster kernel cuts the tensor
+constexpr int kGnClusterSizes[4] = {2, 4, 8, 16};  // 16 needs the non-portable cluster size attribute
+constexpr size_t kGnClusterMaxDyn = 190 * 1024;    // + 33.5 KB static stays under the 227 KB per-CTA limit
+constexpr size_t kGnTwoPerSmDyn = 76 * 1024;       // up to here two CTAs (dynamic + static + 1 KB reserved each) share an SM
+enum { kGnAuto = 0, kGnRendezvous = 1, kGnCluster = 2 };
+struct GnPlan {
+    int kernel;  // kGnRendezvous | kGnCluster
+    int cs;      // cluster size (CTAs that split the rows of one slice)
+    int sc;      // channels per slice: whole groups, a multiple of 8
+    int smem;    // dynamic shared memory per CTA
+    int waves;   // clusters of the launch / clusters the device holds at once, rounded up
 };
-constexpr size_t kGnClusterMaxDyn = 190 * 1024;  // + 33.5 KB static stays under the 227 KB per-CTA limit
-static bool gn_cluster_plan(int NB, int HW, int C, int groups, GnClusterPlan* plan) {
-    const int mode = gn_cluster_mode();
-    if (mode == 0) return false;
+static int g_gn_force[3] = {0, 0, 0};  // imagd_groupnorm_debug_force: kernel, cluster size, slice channels
+static int g_gn_log_on = 0;
+static std::vector<std::pair<std::string, int>> g_gn_log;  // imagd_groupnorm_debug_log
+static std::mutex g_gn_mutex;
+
+template <int CS>
+static cudaError_t gn_cluster_launch(const cudaLaunchConfig_t* cfg, const __nv_bfloat16* x, int64_t ldx, __nv_bfloat16* y,
+                                     int64_t ldy, int HW, int C, int groups, int gps, const float* gamma, const float* beta,
+                                     float eps, int fuse_silu, float* stats_out) {
+    return cudaLaunchKernelEx(cfg, groupnorm_cluster_kernel<CS>, x, ldx, y, ldy, HW, C, groups, gps, gamma, beta, eps,
+                              fuse_silu, stats_out);
+}
+
+// Co-resident clusters of the current device per cluster size, at one and at two CTAs per SM (cap[2 * i + k]: size
+// kGnClusterSizes[i], k + 1 CTAs per SM). A cluster must sit inside one GPC, so this is less than SMs / size and only
+// the occupancy query knows it. Queried once per device; 0 = that cluster size cannot launch.
+template <int CS>
+static int gn_query_capacity(size_t dyn) {
+    if (cudaFuncSetAttribute(groupnorm_cluster_kernel<CS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                             static_cast<int>(kGnClusterMaxDyn)) != cudaSuccess ||
+        (CS > 8 && cudaFuncSetAttribute(groupnorm_cluster_kernel<CS>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) !=
+                       cudaSuccess)) {
+        cudaGetLastError();
+        return 0;
+    }
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3(CS);
+    cfg.blockDim = dim3(kGnThreads);
+    cfg.dynamicSmemBytes = dyn;
+    cudaLaunchAttribute attr;
+    attr.id = cudaLaunchAttributeClusterDimension;
+    attr.val.clusterDim.x = CS;
+    attr.val.clusterDim.y = attr.val.clusterDim.z = 1;
+    cfg.attrs = &attr;
+    cfg.numAttrs = 1;
+    int n = 0;
+    if (cudaOccupancyMaxActiveClusters(&n, groupnorm_cluster_kernel<CS>, &cfg) != cudaSuccess) {
+        cudaGetLastError();
+        return 0;
+    }
+    return n;
+}
+static int gn_device_capacity(int* cap) {
+    static int cache[16][8];
+    static bool have[16];
+    int dev = 0;
+    IMAGD_CUDA(cudaGetDevice(&dev));
+    IMAGD_CHECK_ARG(dev >= 0 && dev < 16, "groupnorm: device index %d", dev);
+    std::lock_guard<std::mutex> lock(g_gn_mutex);
+    if (!have[dev]) {
+        const size_t dyn[2] = {kGnClusterMaxDyn, kGnTwoPerSmDyn};
+        for (int k = 0; k < 2; ++k) {
+            cache[dev][0 + k] = gn_query_capacity<2>(dyn[k]);
+            cache[dev][2 + k] = gn_query_capacity<4>(dyn[k]);
+            cache[dev][4 + k] = gn_query_capacity<8>(dyn[k]);
+            cache[dev][6 + k] = gn_query_capacity<16>(dyn[k]);
+        }
+        have[dev] = true;
+    }
+    memcpy(cap, cache[dev], sizeof(cache[dev]));
+    return IMAGD_OK;
+}
+
+// Predicted microseconds per launch of either kernel. Least-squares fits to tools/gn_bench.py --sweep (every legal plan of
+// the 14 GroupNorm shapes of the UNet step at 512 x 512 batch 1 and 8 and at 768 x 576 batch 8) on an H100 80GB HBM3 SXM
+// at its 700 W limit; each fit is within 35 % of every point; the plan they pick is within 8 % of the fastest candidate at every shape
+// (two batch-8 shapes had a two-wave cluster plan 15-25 % faster than the rendezvous kernel that runs there).
+// mb = bytes read + written in MB.
+//  - cluster, one wave: a CTA's lifetime is a fixed latency chain plus its tile's share of the SM (phase 2 is bound by
+//    the SiLU's two MUFU operations per element, so what counts is the tile bytes per SM: doubled when the clusters only
+//    fit at two CTAs per SM, which also costs ~1 us by itself).
+//  - rendezvous: traffic at the L2 rate up to ~40 MB (the tensor is L2-resident from its producer), at the HBM rate
+//    beyond; wide rows leave few row slots per CTA.
+static double gn_cluster_cost(double mb, int smem, bool two_per_sm) {
+    return 6.32 + 0.0715 * (smem / 1024.0) * (two_per_sm ? 2.0 : 1.0) + 0.0194 * mb + (two_per_sm ? 0.98 : 0.0);
+}
+static double gn_rendezvous_cost(double mb, int C) {
+    return 8.23 + 0.291 * std::min(mb, 40.0) + 0.608 * std::max(mb - 40.0, 0.0) + 2.17 * (C / 1024.0) + (C >= 2560 ? 4.72 : 0.0);
+}
+
+// The plan of one launch from its shape and the device's cluster capacity `cap` (gn_device_capacity layout): the cheapest
+// of the rendezvous kernel and the cluster plans that run as ONE wave (a second wave repeats the whole latency chain, and
+// in the sweep no multi-wave plan beat the rendezvous kernel by more than its fit error). A forced kernel / cluster size /
+// slice width (imagd_groupnorm_debug_force) restricts the candidates, multi-wave plans included; false = none is legal.
+static bool gn_plan(int NB, int HW, int C, int groups, const int* cap, GnPlan* plan) {
     const int cpg = C / groups;
-    // mode 1 keeps to the group widths of the UNet / ControlNet family (10..80 channels), where the kernel was measured and
-    // swept on the GPU; narrower groups (VAE: 4..16 channels, 8..32-byte row pieces per slice) stay on the rendezvous kernel
-    if (mode == 1 && cpg < 10) return false;
-    const int rpc = (HW + kGnCS - 1) / kGnCS;
+    const double mb = 4.0 * NB * HW * C / 1e6;
+    const bool forced_cluster = g_gn_force[0] == kGnCluster || g_gn_force[1] || g_gn_force[2];
     double best = 0.0;
     bool found = false;
-    for (int gps = 1; gps <= groups; ++gps) {
-        if (groups % gps != 0) continue;
-        const int SC = gps * cpg;
-        if (SC % 8 != 0 || SC / 8 > kGnThreads) continue;
-        const size_t tile = static_cast<size_t>(rpc) * SC * 2;
-        const size_t dyn = (3 * static_cast<size_t>(SC) * sizeof(float) + 15) / 16 * 16 + tile;
-        if (dyn > kGnClusterMaxDyn) continue;
-        const int per_sm = (dyn + 35 * 1024) * 2 <= 228 * 1024 ? 2 : 1;
-        const int64_t ctas = static_cast<int64_t>(NB) * (groups / gps) * kGnCS;
-        const int64_t slots = 144LL * per_sm;  // 18 clusters of 8 per CTA slot
-        const int64_t waves = (ctas + slots - 1) / slots;
-        if (mode == 1 && (waves > 1 || tile > 32 * 1024)) continue;
-        // a wave costs a fixed latency chain (~ the time 64 KB take) + its tile; rows under 128 B waste sectors
-        const double cost = static_cast<double>(waves) * (64.0 * 1024 + static_cast<double>(tile) * (SC * 2 < 128 ? 1.3 : 1.0));
-        if (!found || cost < best) {
-            best = cost;
-            plan->gps = gps;
-            plan->smem = dyn;
-            found = true;
+    for (int i = 0; i < 4 && g_gn_force[0] != kGnRendezvous; ++i) {
+        const int cs = kGnClusterSizes[i];
+        if (g_gn_force[1] && g_gn_force[1] != cs) continue;
+        const int rpc = (HW + cs - 1) / cs;
+        for (int gps = 1; gps <= groups; ++gps) {
+            const int sc = gps * cpg;
+            if (groups % gps != 0 || sc % 8 != 0 || (g_gn_force[2] && g_gn_force[2] != sc)) continue;
+            const size_t tile = static_cast<size_t>(rpc) * sc * 2;
+            const size_t dyn = (3 * static_cast<size_t>(sc) * sizeof(float) + 15) / 16 * 16 + tile;
+            if (dyn > kGnClusterMaxDyn) continue;
+            const int64_t clusters = static_cast<int64_t>(NB) * (groups / gps);
+            const bool two_per_sm = clusters > cap[2 * i] && dyn <= kGnTwoPerSmDyn;
+            const int slots = cap[2 * i + (two_per_sm ? 1 : 0)];
+            if (slots <= 0) continue;
+            const int waves = static_cast<int>((clusters + slots - 1) / slots);
+            if (waves > 1 && !forced_cluster) continue;
+            const double cost = waves * gn_cluster_cost(mb, static_cast<int>(dyn), two_per_sm);
+            if (!found || cost < best) {
+                best = cost;
+                *plan = GnPlan{kGnCluster, cs, sc, static_cast<int>(dyn), waves};
+                found = true;
+            }
         }
     }
-    return found;
+    if (forced_cluster) return found;
+    if (found && g_gn_force[0] == kGnAuto && best <= gn_rendezvous_cost(mb, C)) return true;
+    *plan = GnPlan{kGnRendezvous, 0, 0, static_cast<int>(3 * C * sizeof(float)), 1};
+    return true;
 }
 
 template <int VPL, int R>
@@ -627,35 +712,106 @@ int imagd_groupnorm_stats_bf16(const void* x, int64_t ldx, void* y, int64_t ldy,
     IMAGD_CHECK_ARG(groups > 0 && groups <= 64 && C % groups == 0, "groupnorm: groups=%d", groups);
     IMAGD_CHECK_ARG(ldx % 8 == 0 && ldy % 8 == 0 && aligned16(x) && aligned16(y), "groupnorm: alignment");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    GnClusterPlan plan;
-    if (gn_cluster_plan(NB, HW, C, groups, &plan)) {
-        IMAGD_SET_MAX_SMEM(groupnorm_cluster_kernel, static_cast<int>(kGnClusterMaxDyn));
+    int cap[8];
+    int rc = gn_device_capacity(cap);
+    if (rc != IMAGD_OK) return rc;
+    GnPlan plan;
+    IMAGD_CHECK_ARG(gn_plan(NB, HW, C, groups, cap, &plan), "groupnorm: no legal plan for the forced kernel %d cluster %d slice %d",
+                    g_gn_force[0], g_gn_force[1], g_gn_force[2]);
+    if (g_gn_log_on) {  // problem | the plan this launch runs
+        char key[128];
+        snprintf(key, sizeof(key), "%d %d %d %d | %d %d %d %d %d", NB, HW, C, groups, plan.kernel, plan.cs, plan.sc, plan.smem,
+                 plan.waves);
+        std::lock_guard<std::mutex> lock(g_gn_mutex);
+        auto it = std::find_if(g_gn_log.begin(), g_gn_log.end(), [&](const auto& e) { return e.first == key; });
+        if (it == g_gn_log.end()) g_gn_log.emplace_back(key, 1);
+        else ++it->second;
+    }
+    const __nv_bfloat16* xb = reinterpret_cast<const __nv_bfloat16*>(x);
+    __nv_bfloat16* yb = reinterpret_cast<__nv_bfloat16*>(y);
+    if (plan.kernel == kGnCluster) {
         cudaLaunchConfig_t cfg{};
-        cfg.gridDim = dim3(kGnCS * (groups / plan.gps), NB);
+        cfg.gridDim = dim3(plan.cs * (C / plan.sc), NB);
         cfg.blockDim = dim3(kGnThreads);
         cfg.dynamicSmemBytes = plan.smem;
         cfg.stream = st;
         cudaLaunchAttribute attr[2];
         attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = kGnCS;
+        attr[0].val.clusterDim.x = plan.cs;
         attr[0].val.clusterDim.y = 1;
         attr[0].val.clusterDim.z = 1;
         attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
         attr[1].val.programmaticStreamSerializationAllowed = 1;
         cfg.attrs = attr;
         cfg.numAttrs = pdl_enabled() ? 2 : 1;
-        IMAGD_CUDA(cudaLaunchKernelEx(&cfg, groupnorm_cluster_kernel, reinterpret_cast<const __nv_bfloat16*>(x), ldx,
-                                      reinterpret_cast<__nv_bfloat16*>(y), ldy, HW, C, groups, plan.gps, gamma, beta, eps,
-                                      fuse_silu, stats_out));
+        const int gps = plan.sc / (C / groups);
+        switch (plan.cs) {  // (gn_device_capacity opted every instantiation into its shared memory and cluster size)
+            case 2: IMAGD_CUDA(gn_cluster_launch<2>(&cfg, xb, ldx, yb, ldy, HW, C, groups, gps, gamma, beta, eps, fuse_silu, stats_out)); break;
+            case 4: IMAGD_CUDA(gn_cluster_launch<4>(&cfg, xb, ldx, yb, ldy, HW, C, groups, gps, gamma, beta, eps, fuse_silu, stats_out)); break;
+            case 8: IMAGD_CUDA(gn_cluster_launch<8>(&cfg, xb, ldx, yb, ldy, HW, C, groups, gps, gamma, beta, eps, fuse_silu, stats_out)); break;
+            default: IMAGD_CUDA(gn_cluster_launch<16>(&cfg, xb, ldx, yb, ldy, HW, C, groups, gps, gamma, beta, eps, fuse_silu, stats_out)); break;
+        }
         return IMAGD_OK;
     }
     const int chunks = gn_chunks(HW, NB);
-    // 33 KB static + up to 20 KB dynamic (gamma | beta) exceeds the 48 KB default
+    // 33 KB static + up to 30 KB dynamic (gamma | beta | pivots) exceeds the 48 KB default
     IMAGD_SET_MAX_SMEM(groupnorm_fused_kernel, 64 * 1024);
-    IMAGD_CUDA(launch_pdl(groupnorm_fused_kernel, dim3(chunks, NB), dim3(kGnThreads), 3 * C * sizeof(float), st,
-                          reinterpret_cast<const __nv_bfloat16*>(x), ldx, reinterpret_cast<__nv_bfloat16*>(y), ldy, HW, C,
+    IMAGD_CUDA(launch_pdl(groupnorm_fused_kernel, dim3(chunks, NB), dim3(kGnThreads), plan.smem, st, xb, ldx, yb, ldy, HW, C,
                           groups, chunks, reinterpret_cast<float*>(ws) + kGnCounters, gamma, beta, eps, fuse_silu, stats_out));
     return IMAGD_OK;
+}
+
+int imagd_groupnorm_plan(int NB, int HW, int C, int groups, const int* cluster_capacity, int* out) {
+    using namespace imagd;
+    IMAGD_CHECK_ARG(out && NB > 0 && HW > 0 && C > 0 && C % 8 == 0 && C <= kGnMaxC && groups > 0 && groups <= 64 &&
+                        C % groups == 0,
+                    "groupnorm_plan: NB=%d HW=%d C=%d groups=%d", NB, HW, C, groups);
+    int cap[8];
+    if (cluster_capacity) {
+        memcpy(cap, cluster_capacity, sizeof(cap));
+    } else {
+        int rc = gn_device_capacity(cap);
+        if (rc != IMAGD_OK) return rc;
+    }
+    GnPlan plan;
+    IMAGD_CHECK_ARG(gn_plan(NB, HW, C, groups, cap, &plan), "groupnorm_plan: no legal plan for the forced kernel %d cluster %d slice %d",
+                    g_gn_force[0], g_gn_force[1], g_gn_force[2]);
+    const int v[5] = {plan.kernel, plan.cs, plan.sc, plan.smem, plan.waves};
+    memcpy(out, v, sizeof(v));
+    return IMAGD_OK;
+}
+
+int imagd_groupnorm_cluster_capacity(int* out) {
+    IMAGD_CHECK_ARG(out, "groupnorm_cluster_capacity: null pointer");
+    return imagd::gn_device_capacity(out);
+}
+
+int imagd_groupnorm_debug_force(int kernel, int cluster_size, int slice_channels) {
+    IMAGD_CHECK_ARG(kernel >= 0 && kernel <= 2 && (kernel != imagd::kGnRendezvous || (!cluster_size && !slice_channels)),
+                    "groupnorm_debug_force: kernel %d", kernel);
+    IMAGD_CHECK_ARG(cluster_size == 0 || cluster_size == 2 || cluster_size == 4 || cluster_size == 8 || cluster_size == 16,
+                    "groupnorm_debug_force: cluster size %d", cluster_size);
+    IMAGD_CHECK_ARG(slice_channels >= 0 && slice_channels % 8 == 0, "groupnorm_debug_force: slice of %d channels", slice_channels);
+    imagd::g_gn_force[0] = kernel;
+    imagd::g_gn_force[1] = cluster_size;
+    imagd::g_gn_force[2] = slice_channels;
+    return IMAGD_OK;
+}
+
+int imagd_groupnorm_debug_log(int enable, char* out, int out_bytes) {
+    std::lock_guard<std::mutex> lock(imagd::g_gn_mutex);
+    if (enable >= 0) {
+        imagd::g_gn_log_on = enable;
+        if (enable) imagd::g_gn_log.clear();
+    }
+    if (out && out_bytes > 0) {
+        std::string all;
+        for (const auto& k : imagd::g_gn_log) all += k.first + " | " + std::to_string(k.second) + "\n";
+        IMAGD_CHECK_ARG(static_cast<int>(all.size()) < out_bytes, "groupnorm_debug_log: buffer too small (%d needed)",
+                        static_cast<int>(all.size()) + 1);
+        memcpy(out, all.c_str(), all.size() + 1);
+    }
+    return static_cast<int>(imagd::g_gn_log.size());
 }
 
 int imagd_layernorm_bf16(const void* x, int64_t ldx, void* y, int64_t ldy, int rows, int C, const float* gamma,

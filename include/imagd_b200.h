@@ -141,14 +141,27 @@ int imagd_attention_causal_bf16(const void* q, int64_t q_ld, void* out, int64_t 
                                 int head_dim, const imagd_kv_stream* s0, float sm_scale, imagd_stream stream);
 
 /* ---- normalisation ---- */
-/* GroupNorm over [NB, HW, C] (token-major) with optional fused SiLU; workspace ws (imagd_groupnorm_ws_bytes; its first
- * 4 KB are arrival counters that the caller zero-initialises ONCE) holds the per-chunk partial sums. One launch:
- * the CTAs of a sample rendezvous through those counters (grid <= 2 CTAs per SM, so all are co-resident).
+/* GroupNorm over [NB, HW, C] (token-major) with optional fused SiLU, one launch. When the launch fits the device as one
+ * wave of CTA clusters, each cluster keeps a (sample, channel slice) in shared memory: x is read once and the partial
+ * statistics meet in distributed shared memory. Larger launches run a chunked kernel whose CTAs rendezvous through the
+ * workspace ws (imagd_groupnorm_ws_bytes; its first 4 KB are arrival counters that the caller zero-initialises ONCE, the
+ * rest holds per-chunk partial sums; grid <= 2 CTAs per SM, so all are co-resident).
  * Replaces ResnetBlock2D.norm1/norm2 + nonlinearity, Transformer2DModel.norm, conv_norm_out (diffusers-0.24). */
 int64_t imagd_groupnorm_ws_bytes(int NB, int HW, int C, int groups);
 int imagd_groupnorm_bf16(const void* x, int64_t ldx, void* y, int64_t ldy, int NB, int HW, int C, int groups,
                          const float* gamma, const float* beta, float eps, int fuse_silu, void* ws,
                          imagd_stream stream);
+/* The plan imagd_groupnorm_bf16 runs for a shape: out[5] = {kernel (1 chunked rendezvous, 2 cluster), cluster size,
+ * channels per slice, dynamic shared memory per CTA, waves}. cluster_capacity: co-resident clusters per cluster size
+ * 2 / 4 / 8 / 16 at one and at two CTAs per SM ({c2x1, c2x2, c4x1, c4x2, c8x1, c8x2, c16x1, c16x2}, 0 = size not
+ * launchable), or NULL for the current device's (imagd_groupnorm_cluster_capacity). Host-only when the capacity is given. */
+int imagd_groupnorm_plan(int NB, int HW, int C, int groups, const int* cluster_capacity, int* out);
+int imagd_groupnorm_cluster_capacity(int* out);
+/* Test / tuning hooks, as for the GEMM. debug_force: kernel (0 automatic, 1 rendezvous, 2 cluster), cluster size
+ * (0 automatic) and channels per slice (0 automatic) of the next GroupNorm calls; a launch with no legal plan under the
+ * forced values fails. debug_log: "NB HW C groups | kernel cluster slice smem waves | count" per distinct launch. */
+int imagd_groupnorm_debug_force(int kernel, int cluster_size, int slice_channels);
+int imagd_groupnorm_debug_log(int enable, char* out, int out_bytes);
 /* LayerNorm over the last dim of [rows, C]; BasicTransformerBlock.norm1-3 (diffusers-0.24),
  * adapter/resampler.py:16,43-44,187. gamma/beta may be NULL. */
 int imagd_layernorm_bf16(const void* x, int64_t ldx, void* y, int64_t ldy, int rows, int C, const float* gamma,
