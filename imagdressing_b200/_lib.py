@@ -80,6 +80,7 @@ SIGNATURES = {
                                      POINTER(KVStream), POINTER(KVStream), c_float, c_void_p]),
     "imagd_attention_causal_bf16": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_int, c_int, c_int, c_int,
                                             POINTER(KVStream), c_float, c_void_p]),
+    "imagd_attention_debug_force": (c_int, [c_int]),
     "imagd_groupnorm_ws_bytes": (c_int64, [c_int, c_int, c_int, c_int]),
     "imagd_groupnorm_plan": (c_int, [c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "imagd_groupnorm_cluster_capacity": (c_int, [c_void_p]),

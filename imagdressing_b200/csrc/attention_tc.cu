@@ -595,7 +595,19 @@ static int launch_attn_mma(const AttnParams& p, cudaStream_t stream) {
     return IMAGD_OK;
 }
 
+// Test hook (imagd_attention_debug_force): 0 automatic, 1 the mma.sync kernel, 2 the wgmma kernel
+constexpr int kAttnForceMma = 1, kAttnForceWgmma = 2;
+static int g_attn_force = 0;
+
 }  // namespace imagd
+
+extern "C" int imagd_attention_debug_force(int kernel) {
+    using namespace imagd;
+    IMAGD_CHECK_ARG(kernel == 0 || kernel == kAttnForceMma || kernel == kAttnForceWgmma, "attention_debug_force: kernel %d",
+                    kernel);
+    g_attn_force = kernel;
+    return IMAGD_OK;
+}
 
 static int attention_impl(const void* q, int64_t q_ld, void* out, int64_t out_ld, int B, int Lq, int heads, int head_dim,
                           const imagd_kv_stream* s0, const imagd_kv_stream* s1, float sm_scale, int causal,
@@ -667,10 +679,21 @@ static int attention_impl(const void* q, int64_t q_ld, void* out, int64_t out_ld
         IMAGD_CHECK_ARG(!has1 || (aux->out_s0 && aux->out_s1 && aux->ld_s % 8 == 0 && aligned16(aux->out_s0) &&
                                   aligned16(aux->out_s1)),
                         "attention(train): two streams need out_s0 / out_s1");
+        // out_s0 is stored when stream 1 starts, so a sample that skips stream 1 would leave its O_0 rows unwritten;
+        // the backward needs every query sample in both streams anyway
+        IMAGD_CHECK_ARG(!has1 || s1->n_query_samples >= B,
+                        "attention(train): stream 1 must cover every query sample (n_query_samples %d < B %d)",
+                        s1->n_query_samples, B);
         IMAGD_CHECK_ARG(!causal, "attention(train): causal not supported");
     }
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if ((head_dim == 40 || head_dim == 80) && !causal && s0->len >= kAttnWgmmaMinKeys) {
+    const bool wgmma_ok = (head_dim == 40 || head_dim == 80) && !causal;
+    const int force = g_attn_force;
+    IMAGD_CHECK_ARG(force != kAttnForceWgmma || wgmma_ok,
+                    "attention: the wgmma kernel was forced but serves head_dim 40 / 80 non-causal only (head_dim %d%s)",
+                    head_dim, causal ? ", causal" : "");
+    const bool use_wgmma = force == kAttnForceWgmma || (force == 0 && wgmma_ok && s0->len >= kAttnWgmmaMinKeys);
+    if (use_wgmma) {
         const imagd_kv_stream* ws[2] = {s0, has1 ? s1 : nullptr};
         return head_dim == 40 ? launch_attn_wgmma<40>(p, ws, st) : launch_attn_wgmma<80>(p, ws, st);
     }

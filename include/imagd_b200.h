@@ -139,6 +139,10 @@ int imagd_attention_bf16(const void* q, int64_t q_ld, void* out, int64_t out_ld,
  * IMAGDressing_v1_pipeline.py:396-405 encode_prompt). */
 int imagd_attention_causal_bf16(const void* q, int64_t q_ld, void* out, int64_t out_ld, int B, int Lq, int heads,
                                 int head_dim, const imagd_kv_stream* s0, float sm_scale, imagd_stream stream);
+/* Test hook, as for the GEMM: the forward kernel of the next imagd_attention_bf16 / imagd_attention_causal_bf16 /
+ * imagd_attention_train_fwd_bf16 calls (0 automatic, 1 mma.sync, 2 wgmma). A call the forced kernel cannot serve
+ * (wgmma: head_dim 64 / 160 or causal) fails without launching; other values are rejected. */
+int imagd_attention_debug_force(int kernel);
 
 /* ---- normalisation ---- */
 /* GroupNorm over [NB, HW, C] (token-major) with optional fused SiLU, one launch. When the launch fits the device as one
@@ -276,7 +280,8 @@ typedef struct imagd_attn_train {
     int32_t lq_pad;
 } imagd_attn_train;
 
-/* imagd_attention_bf16 + the imagd_attn_train outputs (adapter/attention_processor.py:589-612 under autograd). */
+/* imagd_attention_bf16 + the imagd_attn_train outputs (adapter/attention_processor.py:589-612 under autograd). A second
+ * stream must apply to every query sample (n_query_samples >= B), as the backward requires. */
 int imagd_attention_train_fwd_bf16(const void* q, int64_t q_ld, void* out, int64_t out_ld, int B, int Lq, int heads,
                                    int head_dim, const imagd_kv_stream* s0, const imagd_kv_stream* s1, float sm_scale,
                                    const imagd_attn_train* aux, imagd_stream stream);

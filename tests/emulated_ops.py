@@ -151,7 +151,7 @@ def attention(q, B, Lq, heads, head_dim, s0, s1=None, *, sm_scale=None, out=None
 
     rows = []
     for b in range(B):
-        o = one(s0, b)
+        o = s0.out_scale * one(s0, b)
         if s1 is not None and b < s1.n_query_samples:
             o = o + s1.out_scale * one(s1, b)
         rows.append(o.transpose(0, 1).reshape(Lq, C))

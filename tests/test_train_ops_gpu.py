@@ -75,7 +75,7 @@ def test_attention_backward_matches_autograd(cuda_device, heads, hd, B, L, Lk1, 
     ref = ref_attention(leaves[0], leaves[1], leaves[2], leaves[3] if Lk1 > 0 else None, leaves[4] if Lk1 > 0 else None,
                         heads, 1.0, w1)
     assert rel_l2(out.view(B, L, C), ref) < 1e-2
-    assert rel_l2(out, base) < 4e-3  # the ping-pong kernel serves the inference call at head_dim 40 / 64
+    assert torch.equal(out, base)  # the inference and training forwards run the same kernel
     # log-sum-exp rows (log2 domain) of stream 0
     sp = lambda t: t.reshape(t.shape[0], t.shape[1], heads, hd).transpose(1, 2)
     lse_ref = torch.logsumexp(sp(qf) @ sp(k0f).transpose(-1, -2) * hd ** -0.5, -1) / math.log(2.0)
