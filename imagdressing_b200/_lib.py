@@ -141,6 +141,10 @@ SIGNATURES = {
                                  c_float, c_float, c_int, c_float, c_void_p]),
     "imagd_adamw_step_dev": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_float, c_float, c_float,
                                      c_void_p, c_void_p]),
+    "imagd_grad_norm_ws_bytes": (c_int64, [c_int64]),
+    "imagd_grad_norm_clip": (c_int, [c_void_p, c_int64, c_float, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "imagd_adamw_step_clip": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_float, c_float, c_float,
+                                      c_void_p, c_void_p, c_void_p]),
 }
 
 _lib = None
@@ -178,7 +182,8 @@ LAUNCHES = {"imagd_gemm_bf16": 1, "imagd_conv3x3_bf16": 1, "imagd_upconv3x3_bf16
             "imagd_attention_train_fwd_bf16": 1, "imagd_attention_bwd_prep": 1, "imagd_attention_bwd_bf16": 3,
             "imagd_transpose_bf16": 1, "imagd_conv_weight_layout_bf16": 1, "imagd_conv_weight_flip_bf16": 1, "imagd_im2col3x3_t_bf16": 1, "imagd_col2im3x3_s2_bf16": 1, "imagd_downsum2x_bf16": 1,
             "imagd_colsum_bf16": 2, "imagd_layernorm_bwd_bf16": 3, "imagd_groupnorm_bwd_bf16": 4, "imagd_groupnorm_stats_bf16": 1, "imagd_act_bf16": 1,
-            "imagd_geglu_bf16": 1, "imagd_mse_loss_grad": 2, "imagd_adamw_step": 1, "imagd_adamw_step_dev": 1}
+            "imagd_geglu_bf16": 1, "imagd_mse_loss_grad": 2, "imagd_adamw_step": 1, "imagd_adamw_step_dev": 1,
+            "imagd_grad_norm_clip": 1, "imagd_adamw_step_clip": 1}
 launch_count = 0
 
 

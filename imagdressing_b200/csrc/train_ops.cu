@@ -651,16 +651,20 @@ __global__ void adamw_kernel(float* __restrict__ master, __nv_bfloat16* __restri
 
 // The same with the step-dependent scalars in DEVICE memory — hyper = {lr, weight_decay, step (1-based, as float), grad_scale} —
 // so that a captured CUDA graph of the whole training step replays with a moving step count and learning-rate schedule.
+// CLIP: the update also reads the global-norm state grad_norm_clip_kernel wrote, clip = {norm, coef, finite, skipped}: a
+// non-finite gradient leaves every buffer untouched, otherwise the gradient scale is grad_scale * coef.
+template <bool CLIP>
 __global__ void adamw_dev_kernel(float* __restrict__ master, __nv_bfloat16* __restrict__ param,
                                  const __nv_bfloat16* __restrict__ grad, float* __restrict__ m, float* __restrict__ v, int64_t n,
-                                 float b1, float b2, float eps, const float* __restrict__ hyper) {
+                                 float b1, float b2, float eps, const float* __restrict__ hyper, const double* __restrict__ clip) {
+    if (CLIP && clip[2] == 0.0) return;  // uniform over the grid: the skipped update
     __shared__ float bc[2];
     if (threadIdx.x == 0) {  // the two powf calls once per CTA, not per element
         bc[0] = 1.f - powf(b1, hyper[2]);
         bc[1] = 1.f - powf(b2, hyper[2]);
     }
     __syncthreads();
-    const float lr = hyper[0], wd = hyper[1], gscale = hyper[3];
+    const float lr = hyper[0], wd = hyper[1], gscale = CLIP ? hyper[3] * static_cast<float>(clip[1]) : hyper[3];
     const float bc1 = bc[0], bc2 = bc[1];
     const int64_t i4 = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) * 4;  // four elements per thread, 128-bit accesses
     if (i4 >= n) return;
@@ -698,6 +702,87 @@ __global__ void adamw_dev_kernel(float* __restrict__ master, __nv_bfloat16* __re
             param[i] = __float2bfloat16(w);
         }
     }
+}
+
+// ------------------------------------------------------------------------------------------------ global gradient norm
+// Gradient clipping of the reference's DeepSpeed config ("gradient_clipping": 1.0): the L2 norm of the averaged gradient
+// scale * grad, coef = min(1, max_norm / (norm + 1e-6)), and a finite flag (a non-finite gradient skips the update). Squares
+// add up in fp64: the largest finite bf16 squared is ~1.2e77, so no finite input overflows the sum, and the sum is non-finite
+// exactly when an element is Inf / NaN. Deterministic: one partial per block into `part`, the last block to arrive folds them
+// in a fixed order and resets the arrival counter (graph replays find it at zero). The grid depends on n only.
+constexpr int kNormThreads = 256;
+constexpr int kNormUnroll = 4;  // 128-bit loads in flight per thread
+
+__device__ __forceinline__ double sumsq_bf16x8(const uint4 u, double acc) {
+    const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        const double lo = bf16lo(w[k]), hi = bf16hi(w[k]);
+        acc = fma(lo, lo, acc);
+        acc = fma(hi, hi, acc);
+    }
+    return acc;
+}
+
+// state = {norm, coef, finite (1 / 0), skipped updates}; hyper[2] (the AdamW step count) advances on a finite norm only.
+__global__ void __launch_bounds__(kNormThreads) grad_norm_clip_kernel(const __nv_bfloat16* __restrict__ grad, int64_t n,
+                                                                      float max_norm, float* __restrict__ hyper,
+                                                                      double* __restrict__ state, unsigned int* __restrict__ counter,
+                                                                      double* __restrict__ part) {
+    __shared__ double red[kNormThreads / 32];
+    __shared__ bool last;
+    const int64_t nvec = n / 8;
+    const uint4* g8 = reinterpret_cast<const uint4*>(grad);
+    const int64_t stride = static_cast<int64_t>(gridDim.x) * kNormThreads;
+    int64_t i = static_cast<int64_t>(blockIdx.x) * kNormThreads + threadIdx.x;
+    double acc = 0.0;
+    for (; i + (kNormUnroll - 1) * stride < nvec; i += kNormUnroll * stride) {
+        uint4 u[kNormUnroll];
+#pragma unroll
+        for (int k = 0; k < kNormUnroll; ++k) u[k] = __ldg(g8 + i + k * stride);
+#pragma unroll
+        for (int k = 0; k < kNormUnroll; ++k) acc = sumsq_bf16x8(u[k], acc);
+    }
+    for (; i < nvec; i += stride) acc = sumsq_bf16x8(__ldg(g8 + i), acc);
+    if (blockIdx.x == 0 && threadIdx.x < n - nvec * 8) {  // the < 8 trailing elements
+        const double e = __bfloat162float(grad[nvec * 8 + threadIdx.x]);
+        acc = fma(e, e, acc);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = acc;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double s = 0.0;
+#pragma unroll
+        for (int w = 0; w < kNormThreads / 32; ++w) s += red[w];
+        part[blockIdx.x] = s;
+        __threadfence();
+        last = atomicAdd(counter, 1u) == gridDim.x - 1;
+    }
+    __syncthreads();
+    if (!last || threadIdx.x >= 32) return;
+    __threadfence();
+    double s = 0.0;
+    for (unsigned b = threadIdx.x; b < gridDim.x; b += 32) s += __ldcg(part + b);  // L2: the other blocks' partials
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if (threadIdx.x == 0) {
+        const bool finite = isfinite(s);
+        const double norm = sqrt(s) * static_cast<double>(hyper[3]);
+        state[0] = norm;
+        state[1] = finite ? fmin(1.0, static_cast<double>(max_norm) / (norm + 1e-6)) : 0.0;
+        state[2] = finite ? 1.0 : 0.0;
+        if (finite) hyper[2] += 1.f;
+        else state[3] += 1.0;
+        *counter = 0u;
+    }
+}
+
+static int grad_norm_blocks(int64_t n) {
+    const int64_t per_block = static_cast<int64_t>(kNormThreads) * kNormUnroll * 8;
+    const int64_t b = (n + per_block - 1) / per_block;
+    return static_cast<int>(b < 1 ? 1 : (b > kNumSms * 4 ? kNumSms * 4 : b));
 }
 
 static inline unsigned blocks_for(int64_t n, int threads) { return static_cast<unsigned>((n + threads - 1) / threads); }
@@ -904,8 +989,34 @@ extern "C" int imagd_adamw_step_dev(float* master, void* param, const void* grad
     IMAGD_CHECK_ARG(imagd::aligned16(master) && imagd::aligned16(m) && imagd::aligned16(v) &&
                         (reinterpret_cast<uintptr_t>(param) & 7) == 0 && (reinterpret_cast<uintptr_t>(grad) & 7) == 0,
                     "adamw_dev: buffers must be 16-byte (fp32) / 8-byte (bf16) aligned");
-    adamw_dev_kernel<<<blocks_for((n + 3) / 4, 256), 256, 0, ST(stream)>>>(master, BFW(param), BF(grad), m, v, n, beta1, beta2, eps,
-                                                                          hyper);
+    adamw_dev_kernel<false><<<blocks_for((n + 3) / 4, 256), 256, 0, ST(stream)>>>(master, BFW(param), BF(grad), m, v, n, beta1, beta2,
+                                                                                 eps, hyper, nullptr);
     IMAGD_LAUNCH_CHECK("adamw_dev_kernel");
+    return IMAGD_OK;
+}
+
+extern "C" int64_t imagd_grad_norm_ws_bytes(int64_t n) { return 16 + static_cast<int64_t>(8) * grad_norm_blocks(n); }
+
+extern "C" int imagd_grad_norm_clip(const void* grad, int64_t n, float max_norm, float* hyper, double* state, void* ws,
+                                    imagd_stream stream) {
+    IMAGD_CHECK_ARG(grad && hyper && state && ws && n > 0 && max_norm > 0.f, "grad_norm_clip: bad argument");
+    IMAGD_CHECK_ARG(imagd::aligned16(grad) && imagd::aligned16(ws) && (reinterpret_cast<uintptr_t>(state) & 7) == 0,
+                    "grad_norm_clip: grad / ws must be 16-byte aligned, state 8-byte aligned");
+    grad_norm_clip_kernel<<<grad_norm_blocks(n), kNormThreads, 0, ST(stream)>>>(
+        BF(grad), n, max_norm, hyper, state, static_cast<unsigned int*>(ws),
+        reinterpret_cast<double*>(static_cast<char*>(ws) + 16));
+    IMAGD_LAUNCH_CHECK("grad_norm_clip_kernel");
+    return IMAGD_OK;
+}
+
+extern "C" int imagd_adamw_step_clip(float* master, void* param, const void* grad, float* m, float* v, int64_t n, float beta1,
+                                     float beta2, float eps, const float* hyper, const double* clip_state, imagd_stream stream) {
+    IMAGD_CHECK_ARG(master && param && grad && m && v && hyper && clip_state && n > 0, "adamw_clip: bad argument");
+    IMAGD_CHECK_ARG(imagd::aligned16(master) && imagd::aligned16(m) && imagd::aligned16(v) &&
+                        (reinterpret_cast<uintptr_t>(param) & 7) == 0 && (reinterpret_cast<uintptr_t>(grad) & 7) == 0,
+                    "adamw_clip: buffers must be 16-byte (fp32) / 8-byte (bf16) aligned");
+    adamw_dev_kernel<true><<<blocks_for((n + 3) / 4, 256), 256, 0, ST(stream)>>>(master, BFW(param), BF(grad), m, v, n, beta1, beta2,
+                                                                                eps, hyper, clip_state);
+    IMAGD_LAUNCH_CHECK("adamw_dev_kernel<clip>");
     return IMAGD_OK;
 }

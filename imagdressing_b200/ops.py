@@ -684,3 +684,36 @@ def adamw_step_dev(master: torch.Tensor, param: torch.Tensor, grad: torch.Tensor
     assert hyper.dtype == torch.float32 and hyper.numel() >= 4 and hyper.is_contiguous()
     _lib.check(lib.imagd_adamw_step_dev(master.data_ptr(), param.data_ptr(), grad.data_ptr(), m.data_ptr(), v.data_ptr(), n,
                                         float(beta1), float(beta2), float(eps), hyper.data_ptr(), _stream()), "imagd_adamw_step_dev")
+
+
+def grad_norm_ws_bytes(n: int) -> int:
+    """Bytes of the workspace grad_norm_clip needs for an n-element gradient (allocate once, zeroed)."""
+    return int(_lib.load().imagd_grad_norm_ws_bytes(int(n)))
+
+
+def grad_norm_clip(grad: torch.Tensor, hyper: torch.Tensor, state: torch.Tensor, ws: torch.Tensor, *, max_norm: float) -> None:
+    """Global-norm clipping pass over the flat bf16 gradient: state (fp64 [4]) = {norm of hyper[3] * grad, coef =
+    min(1, max_norm / (norm + 1e-6)), finite, skipped updates}; hyper[2] advances only when the norm is finite. ws: a zeroed
+    uint8 tensor of grad_norm_ws_bytes(grad.numel()) bytes kept for every call (CUDA-graph replayable)."""
+    lib = _lib.load()
+    assert grad.dtype == BF16 and grad.is_contiguous()
+    assert hyper.dtype == torch.float32 and hyper.numel() >= 4 and hyper.is_contiguous()
+    assert state.dtype == torch.float64 and state.numel() >= 4 and state.is_contiguous()
+    assert ws.numel() * ws.element_size() >= grad_norm_ws_bytes(grad.numel())
+    _lib.check(lib.imagd_grad_norm_clip(grad.data_ptr(), grad.numel(), float(max_norm), hyper.data_ptr(), state.data_ptr(),
+                                        ws.data_ptr(), _stream()), "imagd_grad_norm_clip")
+
+
+def adamw_step_clip(master: torch.Tensor, param: torch.Tensor, grad: torch.Tensor, m: torch.Tensor, v: torch.Tensor,
+                    hyper: torch.Tensor, clip_state: torch.Tensor, *, beta1: float, beta2: float, eps: float) -> None:
+    """adamw_step_dev with the gradient scale hyper[3] * coef of grad_norm_clip's state; a non-finite gradient (state
+    finite == 0) leaves master / param / m / v untouched."""
+    lib = _lib.load()
+    n = master.numel()
+    assert master.dtype == torch.float32 and m.dtype == torch.float32 and v.dtype == torch.float32
+    assert param.dtype == BF16 and grad.dtype == BF16 and param.numel() == n and grad.numel() == n
+    assert hyper.dtype == torch.float32 and hyper.numel() >= 4 and hyper.is_contiguous()
+    assert clip_state.dtype == torch.float64 and clip_state.numel() >= 4 and clip_state.is_contiguous()
+    _lib.check(lib.imagd_adamw_step_clip(master.data_ptr(), param.data_ptr(), grad.data_ptr(), m.data_ptr(), v.data_ptr(), n,
+                                         float(beta1), float(beta2), float(eps), hyper.data_ptr(), clip_state.data_ptr(),
+                                         _stream()), "imagd_adamw_step_clip")

@@ -294,19 +294,32 @@ class FlatAdamW:
     accumulation_steps = k (train.py:106-111, :606 `--gradient_accumulation_steps`): k micro-steps share one update. The first
     micro-step's gradients are copied into the flat buffer, the following ones added to it (bf16 sums), the bucket all-reduces
     are launched by the LAST micro-step only, step() returns False without touching the weights until then, and 1/k joins
-    1/world in the kernel's gradient scale."""
+    1/world in the kernel's gradient scale.
+
+    max_grad_norm (None: off) clips the global gradient norm as the reference's DeepSpeed config does ("gradient_clipping":
+    1.0 -> max_grad_norm=1.0): on the window's last micro-step one pass over the whole flat gradient computes the L2 norm of
+    the averaged gradient, the update runs with the gradient scaled by min(1, max_norm / (norm + 1e-6)), and a non-finite
+    gradient skips the update (weights, moments and step count stay as they were). All of it on the device: no host sync, and
+    a captured step graph contains it. Data parallel, every rank holds the whole all-reduced gradient and computes the same
+    norm locally (bit-identical, no extra collective); with shard_states each rank updates its slice with that coefficient.
+    `last_grad_norm` / `skipped_steps` are device scalars for logging (reading them synchronises). Unlike DeepSpeed's fp16
+    overflow path, a skipped update does not hold back the LRScheduler (there is no loss scale in bf16)."""
 
     def __init__(self, params: Iterable[nn.Parameter], lr=1e-4, betas=(0.9, 0.999), eps=1e-8, weight_decay=1e-2,
-                 bucket_bytes: int = 256 << 20, step_fn=None, shard_states: bool = False, accumulation_steps: int = 1):
+                 bucket_bytes: int = 256 << 20, step_fn=None, shard_states: bool = False, accumulation_steps: int = 1,
+                 max_grad_norm: Optional[float] = None):
         seen = set()
         self.params = [p for p in params if p.requires_grad and not (id(p) in seen or seen.add(id(p)))]  # de-duplicated
         assert self.params, "no trainable parameters"
         dev = self.params[0].device
         self.lr, self.betas, self.eps, self.wd = lr, betas, eps, weight_decay
-        self.t = 0
+        self._t = 0
         self.accum = max(1, int(accumulation_steps))
         self._micro = 0  # index of the running micro-step inside its accumulation window
         self._step_fn = step_fn  # test hook with the host-scalar signature of ops.adamw_step; None = the device-scalar kernel
+        if max_grad_norm is not None and (step_fn is not None or not max_grad_norm > 0):
+            raise ValueError("max_grad_norm must be > 0 and runs on the device-scalar kernels (no step_fn)")
+        self.max_grad_norm = None if max_grad_norm is None else float(max_grad_norm)
         # backward produces gradients roughly in reverse registration order: lay the buffer out reversed so that buckets
         # complete front to back
         order = list(reversed(self.params))
@@ -331,6 +344,12 @@ class FlatAdamW:
         # {lr, weight_decay, step, grad_scale} in device memory: what the update kernel reads, so a captured CUDA graph of the
         # step replays with a moving step count / learning-rate schedule (set_lr rewrites it between replays)
         self.hyper = torch.tensor([lr, weight_decay, 0.0, 1.0 / (world * self.accum)], device=dev, dtype=torch.float32)
+        # clipping: {norm, coef, finite, skipped updates} (fp64, ops.grad_norm_clip) and the norm pass's zeroed workspace
+        self.clip_state = self._norm_ws = self.last_grad_norm = self.skipped_steps = None
+        if self.max_grad_norm is not None:
+            self.clip_state = torch.zeros(4, device=dev, dtype=torch.float64)
+            self._norm_ws = torch.zeros(ops.grad_norm_ws_bytes(total), device=dev, dtype=torch.uint8)
+            self.last_grad_norm, self.skipped_steps = self.clip_state[0], self.clip_state[3]
         off = 0
         self._spans = []
         self._gviews = []  # per parameter: its slot of the flat gradient buffer
@@ -419,22 +438,48 @@ class FlatAdamW:
             self._micro += 1
             return False
         self._micro = 0
-        self.t += 1
-        world = (torch.distributed.get_world_size() if self._dist else 1) * self.accum
         lo, hi = self._own
-        self.hyper[2:3].add_(1.0)  # device-side step count (a kernel, so it is part of a captured graph)
-        if self._step_fn is not None:
-            self._step_fn(self.master, self.param[lo:hi], self.grad[lo:hi], self.m, self.v, lr=self.lr, beta1=self.betas[0],
-                          beta2=self.betas[1], eps=self.eps, weight_decay=self.wd, step=self.t, grad_scale=1.0 / world)
+        if self.max_grad_norm is not None:
+            # the norm pass (over the whole buffer: every rank holds the all-reduced gradient) advances the device-side step
+            # count itself, and only for a finite gradient
+            ops.grad_norm_clip(self.grad, self.hyper, self.clip_state, self._norm_ws, max_norm=self.max_grad_norm)
+            ops.adamw_step_clip(self.master, self.param[lo:hi], self.grad[lo:hi], self.m, self.v, self.hyper, self.clip_state,
+                                beta1=self.betas[0], beta2=self.betas[1], eps=self.eps)
         else:
-            ops.adamw_step_dev(self.master, self.param[lo:hi], self.grad[lo:hi], self.m, self.v, self.hyper,
-                               beta1=self.betas[0], beta2=self.betas[1], eps=self.eps)
+            self._t += 1
+            world = (torch.distributed.get_world_size() if self._dist else 1) * self.accum
+            self.hyper[2:3].add_(1.0)  # device-side step count (a kernel, so it is part of a captured graph)
+            if self._step_fn is not None:
+                self._step_fn(self.master, self.param[lo:hi], self.grad[lo:hi], self.m, self.v, lr=self.lr, beta1=self.betas[0],
+                              beta2=self.betas[1], eps=self.eps, weight_decay=self.wd, step=self.t, grad_scale=1.0 / world)
+            else:
+                ops.adamw_step_dev(self.master, self.param[lo:hi], self.grad[lo:hi], self.m, self.v, self.hyper,
+                                   beta1=self.betas[0], beta2=self.betas[1], eps=self.eps)
         if self.shard:  # every rank updated its own slice: gather the bf16 working copy
             torch.distributed.all_gather_into_tensor(self.param, self.param[lo:hi].clone())
         # the kernel wrote through raw pointers: bump the version counters so that weight-derived caches keyed on
         # (data_ptr, _version) — processors._ver, autograd._cached — see the update
         torch.autograd.graph.increment_version([self.param, *self.params])
         return True
+
+    @property
+    def t(self) -> int:
+        """Updates applied so far (AdamW's step count). With clipping it is the device-side count, which a skipped update
+        does not advance: reading it then synchronises."""
+        if self.max_grad_norm is not None:
+            return int(round(float(self.hyper[2])))
+        return self._t
+
+    @t.setter
+    def t(self, value: int) -> None:
+        self._t = int(value)
+        if self.max_grad_norm is not None:
+            self.hyper[2:3].fill_(float(self._t))
+
+    def count_update(self) -> None:
+        """Host side of an update that ran inside a replayed graph (with clipping the device count is the record)."""
+        if self.max_grad_norm is None:
+            self._t += 1
 
     def set_lr(self, lr: float, weight_decay: Optional[float] = None) -> None:
         """Learning-rate schedule hook: rewrites the device-side scalars (outside any graph capture)."""
@@ -451,16 +496,24 @@ class FlatAdamW:
         self.hyper[2:3].zero_()
         self.t = 0
         self._micro = 0
+        if self.clip_state is not None:
+            self.clip_state.zero_()
 
     def state_dict(self) -> Dict[str, object]:
-        return {"t": self.t, "own": self._own, "master": self.master, "m": self.m, "v": self.v,
-                "hyper": dict(lr=self.lr, betas=self.betas, eps=self.eps, weight_decay=self.wd)}
+        sd = {"t": self.t, "own": self._own, "master": self.master, "m": self.m, "v": self.v,
+              "hyper": dict(lr=self.lr, betas=self.betas, eps=self.eps, weight_decay=self.wd)}
+        if self.clip_state is not None:
+            sd["skipped_steps"] = int(self.clip_state[3])
+        return sd
 
     def load_state_dict(self, sd: Dict[str, object]) -> None:
         if tuple(sd["own"]) != tuple(self._own):
             raise ValueError(f"optimizer shard {tuple(sd['own'])} does not match this rank's {self._own}")
         self.t = int(sd["t"])
         self.hyper[2:3].fill_(float(self.t))
+        if self.clip_state is not None:
+            self.clip_state.zero_()
+            self.clip_state[3] = float(sd.get("skipped_steps", 0))
         for name in ("master", "m", "v"):
             getattr(self, name).copy_(sd[name])
         with torch.no_grad():
@@ -711,6 +764,6 @@ class GraphedTrainStep:
         from . import _lib
 
         _lib.launch_count += self.launches_per_step
-        self.opt.t += 1  # (the device-side count advanced inside the graph)
+        self.opt.count_update()  # (the device-side count advanced inside the graph)
         torch.autograd.graph.increment_version([self.opt.param, *self.opt.params])
         return self.loss

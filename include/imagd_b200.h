@@ -355,6 +355,18 @@ int imagd_adamw_step(float* master, void* param, const void* grad, float* m, flo
  * learning-rate schedule — the host only rewrites these four floats. */
 int imagd_adamw_step_dev(float* master, void* param, const void* grad, float* m, float* v, int64_t n, float beta1, float beta2,
                          float eps, const float* hyper, imagd_stream stream);
+/* Global-norm gradient clipping (the reference's DeepSpeed "gradient_clipping"): one deterministic pass over the flat bf16
+ * gradient grad[0:n] writes state (4 doubles) = {norm, coef, finite, skipped}:
+ *   norm = || hyper[3] * grad ||_2 (squares summed in fp64: no finite input overflows), coef = min(1, max_norm / (norm + 1e-6)),
+ *   finite = 1 / 0, skipped += 1 when not finite; hyper[2] (the AdamW step count) += 1 only when finite.
+ * ws: >= imagd_grad_norm_ws_bytes(n) bytes, 16-byte aligned, zeroed once by the caller (an arrival counter the kernel resets
+ * itself, then per-block partials); reused by every call, so one captured CUDA graph replays it. */
+int64_t imagd_grad_norm_ws_bytes(int64_t n);
+int imagd_grad_norm_clip(const void* grad, int64_t n, float max_norm, float* hyper, double* state, void* ws, imagd_stream stream);
+/* imagd_adamw_step_dev reading that state: finite == 0 leaves master, param, m and v untouched; otherwise the update runs
+ * with gradient scale hyper[3] * (float)coef (coef == 1: bitwise the imagd_adamw_step_dev result). */
+int imagd_adamw_step_clip(float* master, void* param, const void* grad, float* m, float* v, int64_t n, float beta1, float beta2,
+                          float eps, const float* hyper, const double* clip_state, imagd_stream stream);
 
 #ifdef __cplusplus
 }
