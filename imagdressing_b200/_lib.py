@@ -111,6 +111,8 @@ SIGNATURES = {
                                                    c_void_p, c_void_p]),
     "imagd_cfg_sampler_step": (c_int, [c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                        c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "imagd_cfg_sampler_pc_step": (c_int, [c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                          c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     # ---- training step (row a13)
     "imagd_attention_train_fwd_bf16": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_int, c_int, c_int, c_int,
                                                POINTER(KVStream), POINTER(KVStream), c_float, POINTER(AttnTrain), c_void_p]),
@@ -179,6 +181,7 @@ LAUNCHES = {"imagd_gemm_bf16": 1, "imagd_conv3x3_bf16": 1, "imagd_upconv3x3_bf16
             "imagd_im2col3x3_s2_bf16": 1, "imagd_im2col3x3_s2_pad_bf16": 1, "imagd_softmax_rows": 1, "imagd_embed_tokens_bf16": 1, "imagd_patchify_bf16": 1, "imagd_broadcast_row_bf16": 1, "imagd_conv3x3_direct_bf16": 1, "imagd_nchw_f32_to_nhwc_bf16": 1,
             "imagd_timestep_embedding": 1, "imagd_linear_small_m": 1, "imagd_cfg_ddim_step": 1,
             "imagd_nchw_f32_to_nhwc_bf16_scaled": 1, "imagd_cfg_sampler_step": 1,
+            "imagd_cfg_sampler_pc_step": 1,
             "imagd_attention_train_fwd_bf16": 1, "imagd_attention_bwd_prep": 1, "imagd_attention_bwd_bf16": 3,
             "imagd_transpose_bf16": 1, "imagd_conv_weight_layout_bf16": 1, "imagd_conv_weight_flip_bf16": 1, "imagd_im2col3x3_t_bf16": 1, "imagd_col2im3x3_s2_bf16": 1, "imagd_downsum2x_bf16": 1,
             "imagd_colsum_bf16": 2, "imagd_layernorm_bwd_bf16": 3, "imagd_groupnorm_bwd_bf16": 4, "imagd_groupnorm_stats_bf16": 1, "imagd_act_bf16": 1,

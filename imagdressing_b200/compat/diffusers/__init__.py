@@ -9,7 +9,7 @@ Never shadow a real diffusers install with this package by accident: it is not o
 """
 from imagdressing_b200.modeling import ControlNetModel, UNet2DConditionModel  # noqa: F401
 from imagdressing_b200.samplers import (DPMSolverMultistepScheduler, EulerAncestralDiscreteScheduler,  # noqa: F401
-                                        EulerDiscreteScheduler)
+                                        EulerDiscreteScheduler, UniPCMultistepScheduler)
 from imagdressing_b200.scheduler import DDIMScheduler  # noqa: F401
 from imagdressing_b200.vae import AutoencoderKL  # noqa: F401
 

@@ -530,6 +530,77 @@ __global__ void cfg_sampler_step_kernel(const float* __restrict__ eps_c, const f
     }
 }
 
+// Predictor-corrector multistep update (UniPC bh1 / bh2, orders 1-3): linear in x, eps and a bank of kPcSlots
+// latents-sized slots (the stash of the previous corrected sample and the previous data predictions), so the scheduler
+// reduces to a per-step row {dx, de, ax, am, a[4], bc, bm, b[4], w_m, w_c} (include/imagd_b200.h).
+constexpr int kPcSlots = 4;
+
+__global__ void cfg_sampler_pc_step_kernel(const float* __restrict__ eps_c, const float* __restrict__ eps_u, float g,
+                                           float* __restrict__ lat, float* __restrict__ bank,
+                                           const float* __restrict__ coef, int32_t* __restrict__ step_ptr,
+                                           const float* __restrict__ mask, const float* __restrict__ img,
+                                           const float* __restrict__ noise, const float* __restrict__ blend_coef,
+                                           int NB, int C, int HW) {
+    pdl_launch_dependents();
+    pdl_wait();
+    unsigned int* done_counter = reinterpret_cast<unsigned int*>(step_ptr + 1);
+    const int step = *step_ptr;
+    const float* row = coef + step * 16;
+    const float dx = row[0], de = row[1], ax = row[2], am = row[3], bc = row[8], bm = row[9];
+    float a[kPcSlots], b[kPcSlots];
+#pragma unroll
+    for (int k = 0; k < kPcSlots; ++k) {
+        a[k] = row[4 + k];
+        b[k] = row[10 + k];
+    }
+    const int w_m = static_cast<int>(row[14]) & (kPcSlots - 1), w_c = static_cast<int>(row[15]) & (kPcSlots - 1);
+    float bn_a = 1.f, bn_b = 0.f;
+    if (mask) {
+        bn_a = blend_coef[step * 2 + 0];
+        bn_b = blend_coef[step * 2 + 1];
+    }
+    const int64_t total = static_cast<int64_t>(NB) * C * HW;
+    for (int64_t idx = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; idx < total;
+         idx += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+        const float u = eps_u ? eps_u[idx] : 0.f;
+        const float c0 = eps_c[idx];
+        const float eps = eps_u ? u + g * (c0 - u) : c0;
+        const float xt = lat[idx];
+        const float m = dx * xt + de * eps;  // this step's data prediction
+        float c = ax * xt + am * m;          // corrected sample
+        float xn = bm * m;
+        // every slot read happens before the two writes below; a slot whose coefficients are both zero is not read
+        // (unwritten slots may hold NaN)
+#pragma unroll
+        for (int k = 0; k < kPcSlots; ++k) {
+            if (a[k] != 0.f || b[k] != 0.f) {
+                const float h = bank[k * total + idx];
+                c += a[k] * h;
+                xn += b[k] * h;
+            }
+        }
+        xn += bc * c;
+        bank[w_m * total + idx] = m;
+        bank[w_c * total + idx] = c;  // the stash holds the corrected sample before any inpaint blend
+        if (mask) {
+            const int64_t n = idx / (static_cast<int64_t>(C) * HW);
+            const float mk = mask[n * HW + idx % HW];
+            const float proper = bn_a * img[idx] + bn_b * noise[idx];
+            xn = (1.f - mk) * proper + mk * xn;
+        }
+        lat[idx] = xn;
+    }
+    __threadfence();
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        const unsigned int prev = atomicAdd(done_counter, 1u);
+        if (prev == gridDim.x - 1) {
+            *done_counter = 0u;
+            *step_ptr = step + 1;
+        }
+    }
+}
+
 // nchw_f32_to_nhwc_bf16 with the model-input scaling of the sigma-space samplers: v * scale[*step_ptr]
 __global__ void nchw_f32_to_nhwc_bf16_scaled_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ y, int NB,
                                                     int C, int H, int W, int Cpad, int repeat,
@@ -734,6 +805,24 @@ int imagd_cfg_sampler_step(const float* eps_cond, const float* eps_uncond, float
     IMAGD_CUDA(launch_pdl(cfg_sampler_step_kernel, dim3(grid), dim3(256), 0, static_cast<cudaStream_t>(stream),
         eps_cond, eps_uncond, guidance, latents, history, step_noise, coef, step_ptr, mask, image_latents, noise,
         blend_coef, NB, C, HW));
+    return IMAGD_OK;
+}
+
+int imagd_cfg_sampler_pc_step(const float* eps_cond, const float* eps_uncond, float guidance, float* latents,
+                              float* bank, const float* coef, int32_t* step_ptr, const float* mask,
+                              const float* image_latents, const float* noise, const float* blend_coef, int NB, int C,
+                              int HW, imagd_stream stream) {
+    using namespace imagd;
+    IMAGD_CHECK_ARG(eps_cond && latents && bank && coef && step_ptr && NB > 0 && C > 0 && HW > 0,
+                    "cfg_sampler_pc_step: bad args");
+    IMAGD_CHECK_ARG(!mask || (image_latents && noise && blend_coef),
+                    "cfg_sampler_pc_step: inpaint blend needs all operands");
+    const int64_t total = static_cast<int64_t>(NB) * C * HW;
+    int grid = grid_for(total, 256);
+    if (grid > kNumSms) grid = kNumSms;
+    IMAGD_CUDA(launch_pdl(cfg_sampler_pc_step_kernel, dim3(grid), dim3(256), 0, static_cast<cudaStream_t>(stream),
+        eps_cond, eps_uncond, guidance, latents, bank, coef, step_ptr, mask, image_latents, noise, blend_coef, NB, C,
+        HW));
     return IMAGD_OK;
 }
 

@@ -9,7 +9,8 @@ Differences that do not change per-sample results (SURVEY.md Appendix B): the tw
 CFG batch [cond.., uncond..] whose first n samples carry the garment stream (B1/B4); the garment pass runs at
 batch n on the garment tokens only (B2); only the 16 attn1 taps are kept (B3); one captured CUDA graph is
 replayed for all steps — the step index lives in device memory and the fused CFG+DDIM kernel (or, for the
-multistep samplers of samplers.py, the generic CFG+sampler-step kernel) advances it.
+multistep samplers of samplers.py, the generic CFG+sampler-step kernel or UniPC's predictor-corrector kernel)
+advances it.
 """
 from __future__ import annotations
 
@@ -111,6 +112,10 @@ class DenoiseEngine:
         if st["ddim"]:
             ops.cfg_ddim_step(eps[:n], eps[n:], st["guidance"], lat, st["coef"], st["step_ptr"], mask=st.get("mask"),
                               image_latents=st.get("image_latents"), noise=st.get("noise"), blend_coef=st.get("blend"))
+        elif "bank" in st:
+            ops.cfg_sampler_pc_step(eps[:n], eps[n:], st["guidance"], lat, st["coef"], st["step_ptr"], st["bank"],
+                                    mask=st.get("mask"), image_latents=st.get("image_latents"), noise=st.get("noise"),
+                                    blend_coef=st.get("blend"))
         else:
             ops.cfg_sampler_step(eps[:n], eps[n:], st["guidance"], lat, st["coef"], st["step_ptr"],
                                  history=st.get("history"), step_noise=st.get("step_noise"), mask=st.get("mask"),
@@ -159,7 +164,8 @@ class DenoiseEngine:
         IMAGDressing_v1_pipeline_ipa_controlnet.py:584-590,643-649); steps with 0 run the UNet without residuals (what
         a zero conditioning scale computes) from a second captured graph. scheduler: the sampler to run (default: the
         one given at construction); DDIMScheduler runs the fused CFG+DDIM kernel, the multistep samplers
-        (samplers.py) the generic sampler-step kernel. step_noise: [S,n,4,h,w], one noise draw per step, for samplers
+        (samplers.py) the generic sampler-step kernel, UniPC the predictor-corrector kernel over a resident slot
+        bank. step_noise: [S,n,4,h,w], one noise draw per step, for samplers
         that add noise (Euler-ancestral). Returns the final latents as a new fp32 tensor."""
         dev = latents.device
         n = latents.shape[0]
@@ -203,6 +209,8 @@ class DenoiseEngine:
                     st.update(history=torch.empty(n, *latents.shape[1:], **f32))
                 if tables.noise:
                     st.update(step_noise=torch.empty(S, n, *latents.shape[1:], **f32))
+                if tables.predictor_corrector:  # one bank for both step graphs; a row reads only slots written before
+                    st.update(bank=torch.empty(ops.PC_SLOTS, n, *latents.shape[1:], **f32))
             if has_control:
                 cp = control_prompt_embeds if control_prompt_embeds is not None else prompt_embeds
                 st.update(control_cond=torch.empty(control_cond.shape, **f32), control_scale=float(control_scale),

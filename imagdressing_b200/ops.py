@@ -383,6 +383,27 @@ def cfg_sampler_step(eps_cond: torch.Tensor, eps_uncond: Optional[torch.Tensor],
     return latents
 
 
+PC_SLOTS = 4
+
+
+def cfg_sampler_pc_step(eps_cond: torch.Tensor, eps_uncond: Optional[torch.Tensor], guidance: float,
+                        latents: torch.Tensor, coef: torch.Tensor, step_ptr: torch.Tensor, bank: torch.Tensor, *,
+                        mask=None, image_latents=None, noise=None, blend_coef=None) -> torch.Tensor:
+    """In-place on `latents` (fp32 NCHW) and `bank` (fp32 [PC_SLOTS, *latents.shape], caller-owned). coef: fp32
+    [S, 16] rows {dx, de, ax, am, a0..a3, bc, bm, b0..b3, w_m, w_c} (include/imagd_b200.h); step_ptr: int32[2]
+    device tensor {step, scratch}."""
+    lib = _lib.load()
+    NB, C, H, W = latents.shape
+    assert latents.dtype == torch.float32 and latents.is_contiguous() and eps_cond.dtype == torch.float32
+    assert step_ptr.dtype == torch.int32 and step_ptr.numel() >= 2 and coef.shape[-1] == 16
+    assert bank.dtype == torch.float32 and bank.shape == (PC_SLOTS, *latents.shape) and bank.is_contiguous()
+    rc = lib.imagd_cfg_sampler_pc_step(eps_cond.data_ptr(), _ptr(eps_uncond), float(guidance), latents.data_ptr(),
+                                       bank.data_ptr(), coef.data_ptr(), step_ptr.data_ptr(), _ptr(mask),
+                                       _ptr(image_latents), _ptr(noise), _ptr(blend_coef), NB, C, H * W, _stream())
+    _lib.check(rc, "imagd_cfg_sampler_pc_step")
+    return latents
+
+
 def embed_tokens(ids: torch.Tensor, tok: torch.Tensor, pos: torch.Tensor) -> torch.Tensor:
     """ids int64 [B, T]; tok bf16 [V, C]; pos bf16 [>= T, C] -> bf16 [B, T, C] = tok[ids] + pos[:T]."""
     lib = _lib.load()

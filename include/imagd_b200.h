@@ -261,6 +261,22 @@ int imagd_cfg_sampler_step(const float* eps_cond, const float* eps_uncond, float
                            float* history, const float* step_noise, const float* coef, int32_t* step_ptr,
                            const float* mask, const float* image_latents, const float* noise, const float* blend_coef,
                            int NB, int C, int HW, imagd_stream stream);
+/* Classifier-free guidance + one predictor-corrector multistep step (UniPCMultistepScheduler bh1 / bh2, orders 1-3,
+ * predict_x0; diffusers-0.24), optionally + the inpainting blend. bank: fp32 [4,NB,C,h,w], four caller-owned slots H[k]
+ * (the host decides which slot holds the stash of the previous corrected sample and which the previous data
+ * predictions). coef: device array [n_steps, 16], row = {dx, de, ax, am, a0..a3, bc, bm, b0..b3, w_m, w_c}; per
+ * element, with eps the CFG-combined output:
+ *   m  = dx x + de eps                          (this step's data prediction)
+ *   c  = ax x + am m + sum_k a_k H[k]           (the corrected sample; ax = 1, the rest 0 without a corrector)
+ *   x' = bc c + bm m + sum_k b_k H[k]           (the predictor)
+ *   H[w_m] = m ; H[w_c] = c                     (slot indices 0..3 stored as floats, written after every read)
+ *   if mask: x' = (1-mask) * (blend[0] img + blend[1] noise) + mask * x'    (c, the stash, is the pre-blend value)
+ * A slot whose a_k and b_k are both zero is not read (an unwritten slot may hold NaN). step_ptr and blend_coef as for
+ * imagd_cfg_ddim_step (the kernel advances the step counter). */
+int imagd_cfg_sampler_pc_step(const float* eps_cond, const float* eps_uncond, float guidance, float* latents,
+                              float* bank, const float* coef, int32_t* step_ptr, const float* mask,
+                              const float* image_latents, const float* noise, const float* blend_coef, int NB, int C,
+                              int HW, imagd_stream stream);
 
 /* ================================================================================================================
  * Training step (SURVEY.md 8 row a13; reference train.py:255-281 SDModel.forward, :573-605 loss + backward, :386-398 AdamW).

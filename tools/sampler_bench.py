@@ -1,10 +1,16 @@
-"""Images/s of the base pipeline (512x512, synthetic SD1.5-shaped weights) per sampler, and the per-launch time of the
-sampler-step kernel next to the CFG+DDIM kernel.
+"""Images/s of the base pipeline (512x512, synthetic SD1.5-shaped weights) per sampler, the per-launch time of the
+sampler-step kernels next to the CFG+DDIM kernel, and the solver error of the few-step samplers.
     python tools/sampler_bench.py [--rounds 3] [--reps 3]
-Arms: DDIM-50, DPM-Solver++ 2M-20, DPM-Solver++ 2M-25, Euler-ancestral-30, at batch 1 and 8. Each round runs every arm
-in turn (a warm-up call that captures the arm's step graph, then `reps` timed calls); rounds alternate the arms so
-clock drift hits them alike. Times are CUDA events around whole pipeline calls (garment pass + denoising loop, output
-latents); the median over rounds is reported. The card name and its power limit are printed with the figures."""
+Arms: DDIM-50, DPM-Solver++ 2M-20, DPM-Solver++ 2M-25, Euler-ancestral-30, UniPC-10 / 15 / 20 (bh2, order 2), at batch
+1 and 8. Each round runs every arm in turn (a warm-up call that captures the arm's step graph, then `reps` timed calls);
+rounds alternate the arms so clock drift hits them alike. Times are CUDA events around whole pipeline calls (garment
+pass + denoising loop, output latents); the median over rounds is reported. The card name and its power limit are
+printed with the figures.
+Accuracy (reported, not asserted): the final-latent rel-L2 of UniPC-10, DPM++2M-10 and DPM++2M-20 against a 250-step
+DPM++2M run of the same random-init pipeline, inputs and seed at batch 1. Every accuracy run uses trailing spacing, so
+all of them integrate the same initial-value problem, from t = 999 down to alphas_cumprod[0] (with the DDIM config's
+leading spacing the first timestep depends on the step count). That is the solver error on this model's
+probability-flow ODE; it says nothing about image quality with trained weights."""
 import argparse
 import json
 import os
@@ -17,10 +23,13 @@ import torch
 
 import bench
 from imagdressing_b200 import ops
-from imagdressing_b200.samplers import DPMSolverMultistepScheduler, EulerAncestralDiscreteScheduler
+from imagdressing_b200.samplers import (DPMSolverMultistepScheduler, EulerAncestralDiscreteScheduler,
+                                        UniPCMultistepScheduler)
 
 ARMS = (("DDIM-50", None, 50), ("DPM++2M-20", DPMSolverMultistepScheduler, 20),
-        ("DPM++2M-25", DPMSolverMultistepScheduler, 25), ("Euler-a-30", EulerAncestralDiscreteScheduler, 30))
+        ("DPM++2M-25", DPMSolverMultistepScheduler, 25), ("Euler-a-30", EulerAncestralDiscreteScheduler, 30),
+        ("UniPC-10", UniPCMultistepScheduler, 10), ("UniPC-15", UniPCMultistepScheduler, 15),
+        ("UniPC-20", UniPCMultistepScheduler, 20))
 
 
 def card():
@@ -44,7 +53,8 @@ def time_call(fn):
 
 def step_kernels(dev, B, launches=100):
     """Mean µs per launch of cfg_ddim_step, of the sampler step with a history row (DPM-Solver++ 2M) and with a noise
-    row (Euler-ancestral), on the CFG batch of B 512x512 latents."""
+    row (Euler-ancestral), and of the predictor-corrector step with a UniPC-20 middle row (corrector and order-2
+    predictor: three slot reads, two slot writes), on the CFG batch of B 512x512 latents."""
     shape = (B, 4, 64, 64)
     eps = torch.randn(2 * B, *shape[1:], device=dev)
     lat, hist = torch.randn(shape, device=dev), torch.zeros(shape, device=dev)
@@ -53,11 +63,16 @@ def step_kernels(dev, B, launches=100):
     ddim = torch.tensor([[0.9, 0.4, 0.95, 0.3]], device=dev).repeat(launches, 1)
     dpm = torch.tensor([[1.1, -0.3, 0.8, 0.1, 0.35, 0.0]], device=dev).repeat(launches, 1)
     ea = torch.tensor([[0.0, 0.0, 1.0, -0.2, 0.0, 0.1]], device=dev).repeat(launches, 1)
+    unipc = UniPCMultistepScheduler()
+    unipc.set_timesteps(20)
+    pc = torch.tensor([unipc._row(5, 5)], device=dev).repeat(launches, 1)
+    bank = torch.randn(ops.PC_SLOTS, *shape, device=dev)
     runs = {"cfg_ddim_step": lambda: ops.cfg_ddim_step(eps[:B], eps[B:], 7.5, lat, ddim, step),
             "cfg_sampler_step (history)": lambda: ops.cfg_sampler_step(eps[:B], eps[B:], 7.5, lat, dpm, step,
                                                                         history=hist),
             "cfg_sampler_step (noise)": lambda: ops.cfg_sampler_step(eps[:B], eps[B:], 7.5, lat, ea, step,
-                                                                      step_noise=z)}
+                                                                      step_noise=z),
+            "cfg_sampler_pc_step (UniPC)": lambda: ops.cfg_sampler_pc_step(eps[:B], eps[B:], 7.5, lat, pc, step, bank)}
     out = {}
     for name, run in runs.items():
         step.zero_()
@@ -69,6 +84,28 @@ def step_kernels(dev, B, launches=100):
             for _ in range(launches):
                 run()
         out[name] = round(time_call(loop) * 1000.0 / launches, 2)
+    return out
+
+
+def accuracy(pipe, ddim, dev):
+    """Final-latent rel-L2 of the few-step arms against DPM++2M-250 on the same inputs and seed (batch 1), all on
+    trailing spacing: the same start (t = 999) and end (alphas_cumprod[0]) for every step count."""
+    x = bench.synth_inputs(1, dev, 0, False, "base", 64, 64)
+
+    def run(cls, steps):
+        pipe.scheduler = cls.from_config(ddim.config, timestep_spacing="trailing")
+        return pipe(prompt=None, null_prompt=None, negative_prompt=None, ref_image=None, width=512, height=512,
+                    num_inference_steps=steps, guidance_scale=bench.GUIDANCE, image_scale=1.0, output_type="latent",
+                    prompt_embeds=x["prompt"], negative_prompt_embeds=x["negative"], latents=x["latents"],
+                    garment_tokens=x["gtok"], ref_image_latents=x["garment"],
+                    generator=torch.Generator().manual_seed(0)).images.float()
+
+    ref = run(DPMSolverMultistepScheduler, 250)
+    out = {}
+    arms = (("UniPC-10", UniPCMultistepScheduler, 10), ("DPM++2M-10", DPMSolverMultistepScheduler, 10),
+            ("DPM++2M-20", DPMSolverMultistepScheduler, 20))
+    for label, cls, steps in arms:
+        out[label] = round(float((run(cls, steps) - ref).norm() / ref.norm()), 5)
     return out
 
 
@@ -111,6 +148,8 @@ def main():
                   f"rounds {[round(t, 1) for t in times[label]]}")
         result["step_kernel_us"][f"B={B}"] = k = step_kernels(dev, B)
         print(f"B={B:<2} step kernels (µs per launch): {k}")
+    result["accuracy_rel_l2_vs_dpm2m_250"] = acc = accuracy(pipe, ddim, dev)
+    print(f"final-latent rel-L2 vs DPM++2M-250 (B=1, random-init weights): {acc}")
     pipe.scheduler = ddim
     print(json.dumps(result))
 
