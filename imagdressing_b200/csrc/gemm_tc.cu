@@ -645,6 +645,8 @@ static int run_gemm_like(const void* A, int64_t lda, int NB, int H, int W, int C
     IMAGD_CHECK_ARG(taps == 1 || Cin % 64 == 0, "conv3x3: Cin=%d must be a multiple of 64", Cin);
     const bool geglu = ep.act == IMAGD_ACT_GEGLU;
     IMAGD_CHECK_ARG(!geglu || N % 128 == 0, "gemm: GEGLU needs packed N %% 128 == 0 (N=%d)", N);
+    IMAGD_CHECK_ARG(!geglu || (!ep.rowvec && !ep.residual && !ep.out_fp32),
+                    "gemm: the GEGLU epilogue takes bias and alpha only (no row vector, residual or fp32 output)");
     IMAGD_CHECK_ARG(ldd % 8 == 0 && aligned16(D), "gemm: output ld=%lld / pointer must be 16-byte aligned", (long long)ldd);
     IMAGD_CHECK_ARG(!ep.residual || (ep.ldr % 8 == 0 && aligned16(ep.residual)), "gemm: residual alignment");
     IMAGD_CHECK_ARG(!ep.bias || aligned16(ep.bias), "gemm: bias alignment");

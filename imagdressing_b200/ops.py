@@ -36,6 +36,33 @@ def _rows2d(t: torch.Tensor) -> Tuple[int, int, int]:
     return rows, t.shape[-1], t.shape[-1]
 
 
+def _pixel_ld(t: torch.Tensor) -> int:
+    """Pixel (row) stride of a channel-last [NB, H, W, C] view whose pixels are equally spaced: a contiguous tensor or a
+    channel slice of a wider NHWC buffer (e.g. the concat buffer of an up block)."""
+    assert t.dim() == 4 and t.stride(-1) == 1, "channel-last [NB, H, W, C] view with contiguous channels"
+    NB, H, W, C = t.shape
+    ld = t.stride(-2)
+    for size, stride, want in ((W, ld, ld), (H, t.stride(-3), W * ld), (NB, t.stride(-4), H * W * ld)):
+        assert size == 1 or stride == want, f"pixels of a {tuple(t.shape)} view with strides {t.stride()} are not equally spaced"
+    assert ld >= C
+    return ld
+
+
+def _conv_epilogue(bias, rowvec, residual, act, NB: int, out: torch.Tensor) -> Epilogue:
+    """Epilogue of a conv launch writing `out` [NB, H, W, Cout]: rowvec [>= NB, >= Cout] fp32 (one row per sample),
+    residual a channel-last view of the output's shape."""
+    _, H, W, Cout = out.shape
+    if rowvec is not None:
+        assert rowvec.dim() == 2 and rowvec.dtype == torch.float32 and rowvec.stride(1) == 1
+        assert rowvec.shape[0] >= NB and rowvec.shape[1] >= Cout, f"rowvec {tuple(rowvec.shape)} for {NB} x {Cout}"
+    ep = _epilogue(bias, rowvec, H * W, None, act, 1.0, False)
+    if residual is not None:
+        assert residual.shape == out.shape and residual.dtype == BF16, f"residual {tuple(residual.shape)} vs {tuple(out.shape)}"
+        ep.residual = residual.data_ptr()
+        ep.ldr = _pixel_ld(residual)
+    return ep
+
+
 class LnFold:
     """LayerNorm folded into the consuming GEMM (include/imagd_b200.h, DESIGN.md section 8): `stats` [M, ld, 2] fp32
     holds the producer's per-row {sum, sum of squares} partials (`parts` of them), `colsum` [N] the column sums of the
@@ -106,16 +133,18 @@ def gemm(a: torch.Tensor, w: torch.Tensor, *, out: Optional[torch.Tensor] = None
 
 def conv3x3(x: torch.Tensor, w: torch.Tensor, *, out: Optional[torch.Tensor] = None, bias=None, rowvec=None,
             residual=None, act: int = ACT_NONE) -> torch.Tensor:
-    """x: [NB, H, W, Cin] bf16 (token-major), w: [Cout, 9*Cin] tap-major. Stride 1, zero pad 1."""
+    """x: [NB, H, W, Cin] bf16 (token-major), w: [Cout, 9*Cin] tap-major. Stride 1, zero pad 1. x, out and residual may
+    be channel slices of wider NHWC buffers (equally spaced pixels); rowvec [>= NB, >= Cout] fp32 is added per sample."""
     lib = _lib.load()
     NB, H, W, Cin = x.shape
-    assert x.is_contiguous() and x.dtype == BF16
+    assert x.dtype == BF16 and w.dtype == BF16
     Cout = w.shape[0]
-    assert w.shape[1] == 9 * Cin
+    assert w.shape[1] == 9 * Cin and w.is_contiguous()
     if out is None:
         out = torch.empty(NB, H, W, Cout, device=x.device, dtype=BF16)
-    ep = _epilogue(bias, rowvec, H * W, residual, act, 1.0, False)
-    rc = lib.imagd_conv3x3_bf16(x.data_ptr(), Cin, NB, H, W, Cin, w.data_ptr(), out.data_ptr(), out.shape[-1], Cout,
+    assert out.shape == (NB, H, W, Cout) and out.dtype == BF16
+    ep = _conv_epilogue(bias, rowvec, residual, act, NB, out)
+    rc = lib.imagd_conv3x3_bf16(x.data_ptr(), _pixel_ld(x), NB, H, W, Cin, w.data_ptr(), out.data_ptr(), _pixel_ld(out), Cout,
                                 ctypes.byref(ep), _stream())
     _lib.check(rc, "imagd_conv3x3_bf16")
     return out
@@ -123,16 +152,18 @@ def conv3x3(x: torch.Tensor, w: torch.Tensor, *, out: Optional[torch.Tensor] = N
 
 def upconv3x3(x: torch.Tensor, w_phase: torch.Tensor, *, bias=None, out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Upsample2D (nearest 2x) + 3x3 conv as four 2x2 phase convs on the low-resolution input (modeling.pack_upconv3x3).
-    x: [NB, H, W, Cin] bf16, w_phase: [4*Cout, 4*Cin] bf16 -> [NB, 2H, 2W, Cout]."""
+    x: [NB, H, W, Cin] bf16, w_phase: [4*Cout, 4*Cin] bf16 -> [NB, 2H, 2W, Cout]; x and out may be channel slices of wider
+    NHWC buffers."""
     lib = _lib.load()
     NB, H, W, Cin = x.shape
-    assert x.is_contiguous() and x.dtype == BF16 and w_phase.dtype == BF16 and w_phase.shape[1] == 4 * Cin
+    assert x.dtype == BF16 and w_phase.dtype == BF16 and w_phase.shape[1] == 4 * Cin and w_phase.is_contiguous()
     Cout = w_phase.shape[0] // 4
     if out is None:
         out = torch.empty(NB, 2 * H, 2 * W, Cout, device=x.device, dtype=BF16)
+    assert out.shape == (NB, 2 * H, 2 * W, Cout) and out.dtype == BF16
     ep = _epilogue(bias, None, 0, None, ACT_NONE, 1.0, False)
-    rc = lib.imagd_upconv3x3_bf16(x.data_ptr(), Cin, NB, H, W, Cin, w_phase.data_ptr(), out.data_ptr(), out.shape[-1], Cout,
-                                  ctypes.byref(ep), _stream())
+    rc = lib.imagd_upconv3x3_bf16(x.data_ptr(), _pixel_ld(x), NB, H, W, Cin, w_phase.data_ptr(), out.data_ptr(), _pixel_ld(out),
+                                  Cout, ctypes.byref(ep), _stream())
     _lib.check(rc, "imagd_upconv3x3_bf16")
     return out
 

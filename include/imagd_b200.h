@@ -41,7 +41,8 @@ int imagd_device_check(void);
 /* ---- fused GEMM / conv epilogue ----
  * out[r, c] = act( alpha * acc[r, c] + bias[c] + rowvec[r / rows_per_group, c] ) + residual[r, c]
  * IMAGD_ACT_GEGLU: the packed weight interleaves, per 128 output rows, 64 "value" rows then their 64 "gate"
- * rows; out has N/2 columns: value * gelu_erf(gate)   (diffusers-0.24 GEGLU in BasicTransformerBlock.ff). */
+ * rows; out has N/2 columns: value * gelu_erf(gate)   (diffusers-0.24 GEGLU in BasicTransformerBlock.ff). It takes
+ * bias and alpha only: a row vector, a residual or an fp32 output is rejected (IMAGD_ERR_ARG). */
 typedef struct imagd_epilogue {
     const float* bias;     /* [N] or NULL */
     const float* rowvec;   /* [groups, rowvec_ld] or NULL (ResnetBlock2D time-embedding add) */
