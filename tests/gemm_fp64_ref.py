@@ -34,7 +34,7 @@ from __future__ import annotations
 
 import math
 from dataclasses import dataclass
-from typing import Optional, Sequence
+from typing import Callable, Optional, Sequence
 
 import torch
 
@@ -292,12 +292,13 @@ def bound(r: Ref) -> torch.Tensor:
 
 
 def check(name: str, got: torch.Tensor, r: Ref, *, bn: int = 128, geom: Optional[Geom] = None, cfg: str = "",
-          family: Optional[str] = None) -> float:
+          family: Optional[str] = None, locate: Optional[Callable[[int, int], str]] = None) -> float:
     """Assert |got - ref| <= bound on every element of got ([rows, cols] after flattening the leading dims); a NaN
     anywhere fails. On failure: the worst element's (row, col), its (m-tile, n-tile) under the launch's pixel box
     (geom; default: 128-row tiles of a GEMM) with `bn` output columns per N tile (64 for GEGLU), the launch
-    configuration `cfg` (the imagd_gemm_debug_log line), the worst-tile and the global rel-L2. Returns the worst
-    (|got - ref| - output rounding allowance) / P, also kept in WORST[family]."""
+    configuration `cfg` (the imagd_gemm_debug_log line), the worst-tile and the global rel-L2. A kernel that is not
+    tiled that way passes `locate(row, col)`, which describes the worst element in the kernel's own terms instead of
+    the tile. Returns the worst (|got - ref| - output rounding allowance) / P, also kept in WORST[family]."""
     ref = r.ref
     cols = ref.shape[-1]
     g = got.detach().reshape(-1, cols).to(ref.device, torch.float64)
@@ -315,6 +316,13 @@ def check(name: str, got: torch.Tensor, r: Ref, *, bn: int = 128, geom: Optional
         return worst_ratio
     flat = int(torch.argmax(excess))
     row, col = divmod(flat, cols)
+    if locate is not None:
+        d2 = torch.nan_to_num((g - ref).square(), nan=math.inf).sum()
+        glob = float((d2 / ref.square().sum().clamp_min(1e-300)).sqrt())
+        raise AssertionError(
+            f"{name}: {n_bad} of {err.numel()} elements out of bound; worst at (row {row}, col {col}), "
+            f"{locate(row, col)} [launch {cfg or '?'}]: got {float(g[row, col])!r}, ref {float(ref[row, col])!r}, "
+            f"bound {float(lim[row, col]):.3e}, E {float(r.E[row, col]):.3e}; global rel-L2 {glob:.3e}")
     geom = geom or Geom(1, 1, ref.shape[0])
     rows = torch.arange(ref.shape[0], device=ref.device)
     mt, phase = geom.tile_of_rows(rows)
