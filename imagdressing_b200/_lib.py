@@ -37,6 +37,9 @@ class Epilogue(Structure):
         ("ln_dim", c_int32),
         ("ln_eps", c_float),
         ("colsum", c_void_p),
+        ("scale_table", c_void_p),
+        ("scale_step", c_void_p),
+        ("scale_ld", c_int64),
     ]
 
 

@@ -211,6 +211,16 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     const int wg = warp >> 2;  // consumer warpgroup: accumulator rows [64 wg, 64 wg + 64)
     const int ct = threadIdx.x;  // consumer thread 0..255
     const imagd_epilogue& ep = p.ep;
+    // Per-step scale (imagd_epilogue.scale_table): two dependent loads issued here, after pdl_wait (the step counter is
+    // advanced by the previous step's sampler kernel), and first used by the epilogue; the second load waits for the first,
+    // which costs these short launches up to about one microsecond (README). s replaces alpha and scales the staged bias; without a table bias_scale = 1 leaves the bias unchanged.
+    float alpha = ep.alpha, bias_scale = 1.0f;
+    if constexpr (LINEAR && LNM == 0) {
+        if (ep.scale_table != nullptr) {
+            const int64_t row = ep.scale_step != nullptr ? static_cast<int64_t>(*ep.scale_step) : 0;
+            alpha = bias_scale = ep.scale_table[row * ep.scale_ld];
+        }
+    }
     // wgmma m64nN accumulator layout: warp w of the warpgroup holds rows 16 w + lane / 4 (+ 8), columns 8 j + 2 (lane % 4)
     // (+ 1); acc[4 j + 2 h + e] is (row frow + 8 h, column 8 j + 2 (lane % 4) + e)
     const int quad = lane & 3;
@@ -351,7 +361,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 
     // ---- epilogue from registers. Per element, in this order: alpha * acc, + bias, + row vector, activation, + residual,
     // round. The LINEAR form always adds bias, row vector and residual (zeros when absent).
-    const float alpha = ep.alpha;
     const bool geglu = !LINEAR && ep.act == IMAGD_ACT_GEGLU;
     const int n_out = geglu ? p.N / 2 : p.N;
     if (geglu) {
@@ -392,6 +401,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             const int cl = 8 * j + 2 * quad;  // tile-local column of element e = 0
             const bool col_ok = col_base + cl < p.N;  // (N % 8 == 0: both elements or neither)
             uint8_t* chunk = epi_chunk(cl / kEpiCols);
+            // s * bias[c], rounded on its own: bitwise the bias the host pre-scaled for an alpha = s launch
+            const float b0 = __fmul_rn(bias_scale, s_bias[cl]), b1 = __fmul_rn(bias_scale, s_bias[cl + 1]);
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 const int r = frow + 8 * h;
@@ -404,8 +415,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                         f[e] = fmaf(ln_rstd[h], fmaf(-ln_mean[h], s_rowvec[cl + e], f[e]), s_bias[cl + e]);
                 } else {
                     if (add_bias) {
-                        f[0] += s_bias[cl];
-                        f[1] += s_bias[cl + 1];
+                        f[0] += b0;
+                        f[1] += b1;
                     }
                     if (add_rowvec) {
                         const float2 v = col_ok ? *reinterpret_cast<const float2*>(rowvec[h] + cl) : make_float2(0.f, 0.f);
@@ -656,6 +667,11 @@ static int run_gemm_like(const void* A, int64_t lda, int NB, int H, int W, int C
     IMAGD_CHECK_ARG(!ep.rowvec || (aligned16(ep.rowvec) && ep.rowvec_ld % 4 == 0 && ep.rows_per_group > 0),
                     "gemm: rowvec alignment / rows_per_group");
     IMAGD_CHECK_ARG(!(ep.row_stats_out && ep.row_stats_in), "gemm: a launch is either a statistics producer or a consumer");
+    IMAGD_CHECK_ARG(!ep.scale_table || (ep.act == IMAGD_ACT_NONE && !ep.rowvec && !ep.out_fp32 && !ep.row_stats_out &&
+                                        !ep.row_stats_in && ep.scale_ld > 0 &&
+                                        (reinterpret_cast<uintptr_t>(ep.scale_table) & 3u) == 0),
+                    "gemm: a scale table needs a plain bf16 epilogue (no activation, row vector, LayerNorm fold, row "
+                    "statistics or fp32 output), scale_ld > 0 and a 4-byte aligned table");
     IMAGD_CHECK_ARG(!ep.row_stats_out || (ep.act == IMAGD_ACT_NONE && !ep.out_fp32 && ep.stats_ld > 0 &&
                                           (reinterpret_cast<uintptr_t>(ep.row_stats_out) & 7u) == 0),
                     "gemm: row_stats_out needs a plain bf16 epilogue, stats_ld > 0 and 8-byte alignment");
@@ -815,6 +831,7 @@ int imagd_gemm_debug_log(int enable, char* out, int out_bytes) {
 int imagd_upconv3x3_bf16(const void* X, int64_t ldx, int NB, int H, int W, int Cin, const void* Wt, void* Y, int64_t ldy,
                          int Cout, const imagd_epilogue* ep, imagd_stream stream) {
     IMAGD_CHECK_ARG(NB > 0 && H > 0 && W > 0 && Cin > 0 && Cout > 0 && Cin % 64 == 0, "upconv3x3: bad shape");
+    IMAGD_CHECK_ARG(!ep || !ep->scale_table, "upconv3x3: the scale table is a GEMM epilogue only");
     IMAGD_CHECK_ARG(!ep || (!ep->rowvec && !ep->residual && ep->act == IMAGD_ACT_NONE && !ep->out_fp32 &&
                             !ep->row_stats_out && !ep->row_stats_in),
                     "upconv3x3: bias-only epilogue");
@@ -841,6 +858,7 @@ int imagd_gemm_debug_timeline(void* device_buf) {
 int imagd_conv3x3_bf16(const void* X, int64_t ldx, int NB, int H, int W, int Cin, const void* Wt, void* Y, int64_t ldy,
                        int Cout, const imagd_epilogue* ep, imagd_stream stream) {
     IMAGD_CHECK_ARG(NB > 0 && H > 0 && W > 0 && Cin > 0 && Cout > 0, "conv3x3: bad shape");
+    IMAGD_CHECK_ARG(!ep || !ep->scale_table, "conv3x3: the scale table is a GEMM epilogue only");
     return imagd::run_gemm_like(X, ldx, NB, H, W, Cin, 9, Wt, static_cast<int64_t>(9) * Cin, Y, ldy, Cout, ep,
                                 static_cast<cudaStream_t>(stream));
 }

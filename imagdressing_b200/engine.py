@@ -35,6 +35,14 @@ class DenoiseEngine:
         self._dummy = {}
         self._zero_t = None
 
+    def _nets(self) -> list:
+        """The ControlNets this engine drives: the `nets` of a MultiControlNetModel, a single ControlNetModel, or none."""
+        from .modeling import MultiControlNetModel
+
+        if self.controlnet is None:
+            return []
+        return list(self.controlnet.nets) if isinstance(self.controlnet, MultiControlNetModel) else [self.controlnet]
+
     # ------------------------------------------------------------------ garment pass
     @torch.no_grad()
     def garment_features(self, ref_latents: torch.Tensor, garment_tokens: torch.Tensor) -> Dict[str, torch.Tensor]:
@@ -88,9 +96,7 @@ class DenoiseEngine:
         with a different `image_scale` / `ipa_scale` / `s_lora_scale` / `c_lora_scale`, or after a
         `load_state_dict`, must not replay the old graph (ADVICE r1, high)."""
         sig = []
-        for model in (self.unet, self.controlnet):
-            if model is None:
-                continue
+        for model in (self.unet, *self._nets()):
             for name, proc in model.attn_processors.items():
                 sig.append((getattr(proc, "scale", None), getattr(proc, "lora_scale", None)))
             sig.append(sum(p._version for p in model.parameters()))
@@ -98,12 +104,22 @@ class DenoiseEngine:
         return tuple(sig)
 
     # ------------------------------------------------------------------ one step
-    def _step(self, st, use_control: bool = True):
+    def _step(self, st, use_control: bool = True, active: tuple = ()):
+        """One step. A single ControlNetModel runs when use_control is set; the nets of a MultiControlNetModel run when
+        their index is in `active`, chained in net order, their zero convs scaled by row step_ptr[0] of st["cn_scale"]."""
         n = st["n"]
         lat = st["latents"]
         table = (st["t_table"], st["step_ptr"])
         down = mid = None
-        if use_control and self.controlnet is not None and st.get("control_cond") is not None:
+        if "cn_scale" in st:
+            nets, res = self._nets(), None
+            for k in active:
+                res = nets[k](lat, None, st["control_text"], st["control_cond"][k], return_dict=False,
+                              timestep_table=table, sample_repeat=2, input_scale=st.get("scale"),
+                              scale_table=st["cn_scale"][:, k], scale_step=st["step_ptr"], residuals=res)
+            if res is not None:
+                down, mid = res
+        elif use_control and self.controlnet is not None and st.get("control_cond") is not None:
             down, mid = self.controlnet(lat, None, st["control_text"], st["control_cond"],
                                         conditioning_scale=st["control_scale"], return_dict=False,
                                         timestep_table=table, sample_repeat=2, input_scale=st.get("scale"))
@@ -131,7 +147,7 @@ class DenoiseEngine:
         n = st["n"]
         jobs = [(self.unet, st["text"], st["kwargs"])]
         if self.controlnet is not None and st.get("control_cond") is not None:
-            jobs.append((self.controlnet, st["control_text"], {}))
+            jobs += [(net, st["control_text"], {}) for net in self._nets()]
         for model, _, _ in jobs:
             for m in model.modules():
                 if isinstance(m, Attention) and not hasattr(m.processor, "_kv2_memo"):
@@ -147,7 +163,9 @@ class DenoiseEngine:
                                                                        dtype=torch.bfloat16)
                     proc(m, dummy, encoder_hidden_states=text if m.is_cross else None, _prepare_only=True, **kw)
         if len(jobs) > 1:
-            self.controlnet.cond_embedding(st["control_cond"], 2 * n)
+            conds = st["control_cond"] if "cn_scale" in st else [st["control_cond"]]
+            for net, cond in zip(self._nets(), conds):
+                net.cond_embedding(cond, 2 * n)
         return True
 
     # ------------------------------------------------------------------ sampling
@@ -170,7 +188,13 @@ class DenoiseEngine:
         bank. step_noise: [S,n,4,h,w], one noise draw per step, for samplers
         that add noise (Euler-ancestral). adapter_states: the four T2I-Adapter features of this call (token-major bf16
         [1 or n, h, w, C], or NCHW), added to both CFG halves at every step times adapter_conditioning_scale; the scale
-        lives in device memory, so changing it replays the same graph. Returns the final latents as a new fp32 tensor."""
+        lives in device memory, so changing it replays the same graph. Returns the final latents as a new fp32 tensor.
+
+        With a MultiControlNetModel of K nets, control_cond is a list of K images (batch 1 or n each), control_scale a
+        list of K floats and control_keep None or a list of K per-step 0/1 lists. The scales times the keeps are staged
+        into a resident [S, K] table that the zero convs read on the device, so new scales replay the same graphs. Steps
+        are grouped by their active set (the nets kept at that step); each distinct set has its own step graph, captured
+        on first use into the memory pool of the first one, which runs only those nets, chained in net order."""
         dev = latents.device
         n = latents.shape[0]
         sch = scheduler if scheduler is not None else self.scheduler
@@ -192,15 +216,31 @@ class DenoiseEngine:
             return t if t.shape[0] == n else t.expand(n, -1, -1)
 
         has_control = self.controlnet is not None and control_cond is not None
+        from .modeling import MultiControlNetModel
+
+        multi = has_control and isinstance(self.controlnet, MultiControlNetModel)
+        if multi:
+            K = len(self.controlnet.nets)
+            control_cond, control_scale = list(control_cond), [float(s) for s in control_scale]
+            keeps = [[1.0] * S] * K if control_keep is None else [[float(k) for k in kk] for kk in control_keep]
+            if len(control_cond) != K or len(control_scale) != K or len(keeps) != K:
+                raise ValueError(f"{len(control_cond)} images, {len(control_scale)} scales and {len(keeps)} guidance "
+                                 f"windows for {K} ControlNets")
+            if any(len(kk) != S or any(k not in (0.0, 1.0) for k in kk) for kk in keeps):
+                raise ValueError("control_keep must hold one 0/1 entry per step for each ControlNet")
+            active = [tuple(k for k in range(K) if keeps[k][i] > 0) for i in range(S)]
         if adapter_states is not None:
             adapter_states = self.unet.adapter_tokens(adapter_states, latents.shape[-2:])
             if any(f.shape[0] not in (1, n) for f in adapter_states):
                 raise ValueError(f"adapter features must hold 1 or {n} samples")
+        cond_shape = None
+        if has_control:
+            cond_shape = tuple(tuple(c.shape) for c in control_cond) if multi else tuple(control_cond.shape)
         key = (n, tuple(latents.shape[1:]), prompt_embeds.shape[1], has_control, mask is not None,
-               float(guidance_scale), float(control_scale), bool(sa_hidden_states), id(t_table), id(coef),
-               tuple(control_cond.shape) if has_control else None, self._frozen_signature(),
+               float(guidance_scale), None if multi else float(control_scale), bool(sa_hidden_states), id(t_table),
+               id(coef), cond_shape, self._frozen_signature(),
                tuple(tuple(f.shape) for f in adapter_states) if adapter_states is not None else None)
-        keep = [1.0] * S if control_keep is None or not has_control else [float(k) for k in control_keep]
+        keep = [1.0] * S if control_keep is None or not has_control or multi else [float(k) for k in control_keep]
         if len(keep) != S or any(k not in (0.0, 1.0) for k in keep):
             raise ValueError("control_keep must hold one 0/1 entry per step")
         st = self._states.get(key)
@@ -222,8 +262,12 @@ class DenoiseEngine:
                     st.update(bank=torch.empty(ops.PC_SLOTS, n, *latents.shape[1:], **f32))
             if has_control:
                 cp = control_prompt_embeds if control_prompt_embeds is not None else prompt_embeds
-                st.update(control_cond=torch.empty(control_cond.shape, **f32), control_scale=float(control_scale),
-                          control_text=torch.empty(2 * n, cp.shape[1], cp.shape[2], device=dev, dtype=torch.bfloat16))
+                st.update(control_text=torch.empty(2 * n, cp.shape[1], cp.shape[2], device=dev, dtype=torch.bfloat16))
+                if multi:  # graphs: active set -> (graph, launches); pool: the first capture's memory pool
+                    st.update(control_cond=[torch.empty(c.shape, **f32) for c in control_cond],
+                              cn_scale=torch.empty(S, K, **f32), graphs={}, pool=None)
+                else:
+                    st.update(control_cond=torch.empty(control_cond.shape, **f32), control_scale=float(control_scale))
             if mask is not None:
                 st.update(mask=torch.empty(mask.shape, **f32), image_latents=torch.empty(image_latents.shape, **f32),
                           noise=torch.empty(noise.shape, **f32), blend=blend)
@@ -240,7 +284,13 @@ class DenoiseEngine:
         if has_control:
             cp = control_prompt_embeds if control_prompt_embeds is not None else prompt_embeds
             cn = control_negative_embeds if control_negative_embeds is not None else negative_prompt_embeds
-            st["control_cond"].copy_(control_cond)
+            if multi:
+                for buf, c in zip(st["control_cond"], control_cond):
+                    buf.copy_(c)
+                st["cn_scale"].copy_(torch.tensor([[control_scale[k] * keeps[k][i] for k in range(K)] for i in range(S)],
+                                                  dtype=torch.float32))
+            else:
+                st["control_cond"].copy_(control_cond)
             st["control_text"][:n].copy_(bn(cp))
             st["control_text"][n:].copy_(bn(cn))
         if mask is not None:
@@ -265,7 +315,7 @@ class DenoiseEngine:
 
         if not (self.use_cuda_graph and dev.type == "cuda") or callback is not None:
             for i in range(S):
-                self._step(st, use_control=keep[i] > 0)
+                self._step(st, use_control=keep[i] > 0, active=active[i] if multi else ())
                 if callback is not None:
                     callback(i, int(timesteps[i]), lat)
             return lat.clone()
@@ -274,6 +324,8 @@ class DenoiseEngine:
         # conditioning embedding) — recomputed IN PLACE, so the device addresses the captured graph holds stay
         # valid. The first call for a configuration runs one full eager step instead (packs weights, sizes
         # workspaces) and then captures the step graph, which is replayed for every step of every later image.
+        if multi:
+            return self._sample_multi(st, active)
         if st["graph"] is None or not self._refresh(st):
             self._step(st)
             lat.copy_(st["lat0"])
@@ -303,4 +355,30 @@ class DenoiseEngine:
             else:
                 st["graph_nc"].replay()
                 _lib.launch_count += st["graph_nc_launches"]
+        return lat.clone()
+
+    def _sample_multi(self, st, active: List[tuple]) -> torch.Tensor:
+        """The graph-replayed loop of a MultiControlNetModel: one step graph per distinct active set."""
+        lat = st["latents"]
+        graphs = st["graphs"]
+        if not graphs or not self._refresh(st):
+            self._step(st, active=tuple(range(len(self._nets()))))  # every net: packs weights, sizes workspaces
+            lat.copy_(st["lat0"])
+            st["step_ptr"].zero_()
+        for a in dict.fromkeys(active):  # distinct active sets, in order of first use
+            if a in graphs:
+                continue
+            torch.cuda.synchronize()
+            graph = torch.cuda.CUDAGraph()
+            before = _lib.launch_count
+            with torch.cuda.graph(graph, pool=st["pool"]):  # the sets' steps never overlap: one activation pool
+                self._step(st, active=a)
+            graphs[a] = (graph, _lib.launch_count - before)
+            _lib.launch_count = before
+            if st["pool"] is None:
+                st["pool"] = graph.pool()
+        for a in active:
+            graph, launches = graphs[a]
+            graph.replay()
+            _lib.launch_count += launches
         return lat.clone()

@@ -912,7 +912,13 @@ class ControlNetModel(_ModelBase):
     def forward(self, sample, timestep, encoder_hidden_states, controlnet_cond, conditioning_scale: float = 1.0,
                 class_labels=None, timestep_cond=None, attention_mask=None, added_cond_kwargs=None,
                 cross_attention_kwargs=None, guess_mode: bool = False, return_dict: bool = True,
-                timestep_table=None, sample_repeat: int = 1, input_scale=None):
+                timestep_table=None, sample_repeat: int = 1, input_scale=None, scale_table=None, scale_step=None,
+                residuals=None):
+        """scale_table / scale_step / residuals: the multi-ControlNet path (MultiControlNetModel, DenoiseEngine). The 13
+        zero convs then read their scale on the device from scale_table (an fp32 column view [S, K][:, k]) at row
+        scale_step[0] (row 0 without a step pointer) instead of the host float conditioning_scale, and each adds the
+        matching residual of `residuals` = (down list, mid) - the previous net's outputs - so the last net of a chain
+        returns the sum of all of them, rounded to bf16 once per net."""
         assert not guess_mode, "guess_mode is False in every reference script (SURVEY.md B14)"
         pk = self._cn_packed()
         NB = sample.shape[0] * sample_repeat
@@ -926,6 +932,12 @@ class ControlNetModel(_ModelBase):
             x, outs = blk.run(x, temb_all, ctx, cross_attention_kwargs or {})
             skips += outs
         x = self.mid_block.run(x, temb_all, ctx, cross_attention_kwargs or {})
+        if scale_table is not None:
+            prev_down, prev_mid = residuals if residuals is not None else ([None] * len(skips), None)
+            tab = dict(scale_table=scale_table, scale_step=scale_step)
+            down = [ops.gemm(t, w, bias=b, residual=r, **tab) for t, w, b, r in zip(skips, pk["zw"], pk["zb"], prev_down)]
+            mid = ops.gemm(x, pk["mw"], bias=pk["mb"], residual=prev_mid, **tab)
+            return (down, mid) if not return_dict else ControlNetOutput(down, mid)
         s = float(conditioning_scale)
         sb = pk.get(("scaled", s))
         if sb is None:  # conditioning_scale folded into the 1x1 "zero conv" epilogues: alpha * acc + (s * bias)
@@ -944,6 +956,66 @@ class ControlNetOutput:
 
     def __iter__(self):
         return iter((self.down_block_res_samples, self.mid_block_res_sample))
+
+
+class MultiControlNetModel(nn.Module):
+    """diffusers-0.24 MultiControlNetModel (pipelines/controlnet/multicontrolnet.py): several ControlNets in one call,
+    their residuals summed. `nets` is a ModuleList, so state_dict keys are `nets.{k}.*` and .to() moves every net.
+    Each net's zero convs add the previous net's outputs in their epilogue (ControlNetModel.forward `residuals=`), so
+    the sum costs no extra pass; it is rounded to bf16 once per net where diffusers rounds twice (output, then sum)."""
+
+    def __init__(self, controlnets):
+        super().__init__()
+        nets = list(controlnets)
+        if not nets or not all(isinstance(n, ControlNetModel) for n in nets):
+            raise ValueError("MultiControlNetModel takes a non-empty list of ControlNetModel")
+        if len({id(n) for n in nets}) != len(nets):
+            # one module object holds one cached conditioning embedding: two images cannot share it
+            raise ValueError("each ControlNetModel object may appear once in a MultiControlNetModel")
+        self.nets = nn.ModuleList(nets)
+
+    @property
+    def attn_processors(self) -> Dict[str, object]:
+        return {f"nets.{k}.{name}": p for k, net in enumerate(self.nets) for name, p in net.attn_processors.items()}
+
+    @property
+    def config(self):
+        return self.nets[0].config
+
+    @property
+    def dtype(self) -> torch.dtype:
+        return self.nets[0].dtype
+
+    @property
+    def device(self) -> torch.device:
+        return self.nets[0].device
+
+    def load_state_dict(self, state_dict, strict: bool = True, **kw):
+        out = super().load_state_dict(state_dict, strict=strict, **kw)
+        self.invalidate_packed()
+        return out
+
+    def invalidate_packed(self):
+        for net in self.nets:
+            net.invalidate_packed()
+
+    @torch.no_grad()
+    def forward(self, sample, timestep, encoder_hidden_states, controlnet_cond: List[torch.Tensor],
+                conditioning_scale: List[float], class_labels=None, timestep_cond=None, attention_mask=None,
+                added_cond_kwargs=None, cross_attention_kwargs=None, guess_mode: bool = False, return_dict: bool = True,
+                timestep_table=None, sample_repeat: int = 1, input_scale=None):
+        """Returns the summed (down residuals, mid residual) as diffusers does. The scales are staged into a [1, K]
+        device table that the zero convs read."""
+        K = len(self.nets)
+        if len(controlnet_cond) != K or len(conditioning_scale) != K:
+            raise ValueError(f"{len(controlnet_cond)} images and {len(conditioning_scale)} scales for {K} ControlNets")
+        table = torch.tensor([[float(s) for s in conditioning_scale]], dtype=torch.float32, device=sample.device)
+        res = None
+        for k, (net, image) in enumerate(zip(self.nets, controlnet_cond)):
+            res = net(sample, timestep, encoder_hidden_states, image, cross_attention_kwargs=cross_attention_kwargs,
+                      guess_mode=guess_mode, return_dict=False, timestep_table=timestep_table,
+                      sample_repeat=sample_repeat, input_scale=input_scale, scale_table=table[:, k], residuals=res)
+        return res
 
 
 def init_synthetic_(model: nn.Module, seed: int = 0) -> nn.Module:

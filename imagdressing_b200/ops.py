@@ -98,10 +98,19 @@ def _epilogue(bias, rowvec, rows_per_group, residual, act, alpha, out_fp32) -> E
 
 def gemm(a: torch.Tensor, w: torch.Tensor, *, out: Optional[torch.Tensor] = None, bias=None, rowvec=None,
          rows_per_group: int = 0, residual=None, act: int = ACT_NONE, alpha: float = 1.0,
-         out_fp32: bool = False, stats_out: Optional[torch.Tensor] = None, ln: Optional[LnFold] = None) -> torch.Tensor:
+         out_fp32: bool = False, stats_out: Optional[torch.Tensor] = None, ln: Optional[LnFold] = None,
+         scale_table: Optional[torch.Tensor] = None, scale_step: Optional[torch.Tensor] = None) -> torch.Tensor:
     """out[M, N] = epilogue(a[M, K] @ w[N, K]^T); a / w / residual bf16, bias / rowvec fp32.
     stats_out [M, ld, 2] fp32: also emit per-row {sum, sum of squares} of the rounded outputs, one slot per N tile.
-    ln: the rows of `a` are the RAW input of a LayerNorm that has been folded into `w` / `bias` (LnFold)."""
+    ln: the rows of `a` are the RAW input of a LayerNorm that has been folded into `w` / `bias` (LnFold).
+    scale_table: fp32 device column view [S, K][:, k] (or a 1-D [S] table); the kernel reads s = scale_table[scale_step[0]]
+    (row 0 without scale_step, an int32 device tensor) and computes s * acc + s * bias + residual in place of alpha."""
+    if scale_table is not None:  # the kernel sees only a pointer: dtype, rank and device are checked here
+        if scale_table.dtype != torch.float32 or scale_table.dim() != 1 or not scale_table.is_cuda:
+            raise ValueError(f"scale_table must be a 1-D fp32 CUDA tensor (a column view [S, K][:, k]), got "
+                             f"{scale_table.dtype} {tuple(scale_table.shape)} on {scale_table.device}")
+        if scale_step is not None and (scale_step.dtype != torch.int32 or not scale_step.is_cuda):
+            raise ValueError(f"scale_step must be an int32 CUDA tensor, got {scale_step.dtype} on {scale_step.device}")
     lib = _lib.load()
     M, K, lda = _rows2d(a)
     N, Kw = w.shape
@@ -125,6 +134,10 @@ def gemm(a: torch.Tensor, w: torch.Tensor, *, out: Optional[torch.Tensor] = None
         ep.ln_dim = ln.dim
         ep.ln_eps = ln.eps
         ep.colsum = ln.colsum.data_ptr()
+    if scale_table is not None:
+        ep.scale_table = scale_table.data_ptr()
+        ep.scale_step = _ptr(scale_step)
+        ep.scale_ld = scale_table.stride(0)
     rc = lib.imagd_gemm_bf16(a.data_ptr(), lda, w.data_ptr(), w.stride(0), out.data_ptr(), ldd, M, N, K,
                              ctypes.byref(ep), _stream())
     _lib.check(rc, "imagd_gemm_bf16")

@@ -9,7 +9,10 @@ every edge can be bypassed with precomputed tensors (`prompt_embeds`, `negative_
 `ref_image_latents`, `output_type="latent"`), which is how the offline benchmark and tests drive it.
 
 Extensions over the reference (which hard-codes batch 1, SURVEY.md B1): any batch n = latents / prompt_embeds
-batch or `num_images_per_prompt`; per-sample or shared (batch-1, broadcast) garment.
+batch or `num_images_per_prompt`; per-sample or shared (batch-1, broadcast) garment. The two pose pipelines also accept
+several ControlNets (a MultiControlNetModel or a list), which the reference normalises the arguments for and then
+asserts on: one pose image, scale and guidance window per net, the nets' residuals summed, as its inpainting pipeline
+(and diffusers' StableDiffusionControlNetPipeline) does.
 """
 from __future__ import annotations
 
@@ -18,6 +21,7 @@ from typing import Any, Callable, Dict, List, Optional, Union
 import torch
 
 from .engine import DenoiseEngine
+from .modeling import MultiControlNetModel
 
 
 class StableDiffusionPipelineOutput:
@@ -48,6 +52,30 @@ def _control_window(guess_mode, start, end):
     if not 0.0 <= start <= end <= 1.0:
         raise ValueError(f"control guidance window [{start}, {end}] must satisfy 0 <= start <= end <= 1")
     return start, end
+
+
+def _multi_control_args(K: int, guess_mode, images, scale, start, end):
+    """The per-net lists of a K-net MultiControlNetModel call: a float scale is broadcast, and a scalar guidance start /
+    end is repeated to the other's length or to K, as the reference normalises them (ipa_controlnet.py:443-454). Every
+    window is checked as _control_window checks one."""
+    as_list = lambda v: list(v) if isinstance(v, (list, tuple)) else v
+    start, end, scale = as_list(start), as_list(end), as_list(scale)
+    if not isinstance(start, list) and isinstance(end, list):
+        start = len(end) * [start]
+    elif not isinstance(end, list) and isinstance(start, list):
+        end = len(start) * [end]
+    elif not isinstance(start, list) and not isinstance(end, list):
+        start, end = K * [start], K * [end]
+    if not isinstance(scale, list):
+        scale = K * [scale]
+    if not isinstance(images, (list, tuple)):
+        raise ValueError(f"a MultiControlNetModel of {K} nets takes a list of {K} control images")
+    for name, v in (("control images", images), ("controlnet_conditioning_scale", scale),
+                    ("control_guidance_start", start), ("control_guidance_end", end)):
+        if len(v) != K:
+            raise ValueError(f"{len(v)} {name} for {K} ControlNets")
+    windows = [_control_window(guess_mode, s, e) for s, e in zip(start, end)]
+    return list(images), [float(v) for v in scale], [w[0] for w in windows], [w[1] for w in windows]
 
 
 def _image_batch(image, width, height, *, gray: bool = False) -> torch.Tensor:
@@ -325,9 +353,12 @@ class _DressingPipelineBase:
                                                   latents.shape[-2] * self.vae_scale_factor, device)
 
         keep = None
-        if control_image is not None and (control_guidance_start != 0.0 or control_guidance_end != 1.0):
-            T = len(timesteps)  # controlnet_keep, ipa_controlnet.py:584-590 / inpainting.py:373-379
-            keep = [1.0 - float(i / T < control_guidance_start or (i + 1) / T > control_guidance_end) for i in range(T)]
+        T = len(timesteps)  # controlnet_keep, ipa_controlnet.py:584-590 / inpainting.py:373-379
+        window = lambda start, end: [1.0 - float(i / T < start or (i + 1) / T > end) for i in range(T)]
+        if isinstance(control_image, list):  # MultiControlNetModel: one window per net
+            keep = [window(s, e) for s, e in zip(control_guidance_start, control_guidance_end)]
+        elif control_image is not None and (control_guidance_start != 0.0 or control_guidance_end != 1.0):
+            keep = window(control_guidance_start, control_guidance_end)
         out = self._engine.sample(
             latents, prompt_embeds, negative_prompt_embeds, sa, guidance_scale, len(timesteps), timesteps=timesteps,
             control_keep=keep,
@@ -379,6 +410,8 @@ class IMAGDressing_v1_ControlNet(_DressingPipelineBase):
 
     def __init__(self, vae, reference_unet, unet, tokenizer, text_encoder, controlnet, image_encoder, ImgProj, scheduler,
                  safety_checker=None, feature_extractor=None, requires_safety_checker: bool = False, adapter=None):
+        if isinstance(controlnet, (list, tuple)):  # as StableDiffusionControlNetPipeline.__init__ (diffusers-0.24)
+            controlnet = MultiControlNetModel(controlnet)
         self.register_modules(vae=vae, reference_unet=reference_unet, unet=unet, controlnet=controlnet,
                               scheduler=scheduler, tokenizer=tokenizer, text_encoder=text_encoder,
                               image_encoder=image_encoder, ImgProj=ImgProj, safety_checker=safety_checker,
@@ -391,6 +424,16 @@ class IMAGDressing_v1_ControlNet(_DressingPipelineBase):
             return image.to(device=device, dtype=torch.float32)
         return _image_batch(image, width, height).to(device)  # control_image_processor: lanczos, no normalisation
 
+    def _control_inputs(self, guess_mode, image, scale, start, end, width, height):
+        """(prepared control image(s), scale(s), guidance start(s), end(s)): scalars for a ControlNetModel, per-net lists
+        for a MultiControlNetModel."""
+        dev = self._execution_device
+        if isinstance(self.controlnet, MultiControlNetModel):
+            images, scale, start, end = _multi_control_args(len(self.controlnet.nets), guess_mode, image, scale, start, end)
+            return [self.prepare_image(im, width, height, dev) for im in images], scale, start, end
+        start, end = _control_window(guess_mode, start, end)
+        return (self.prepare_image(image, width, height, dev) if image is not None else None), float(scale), start, end
+
     def __call__(self, prompt, null_prompt, negative_prompt, ref_image, width, height, num_inference_steps,
                  guidance_scale, pose_image=None, ref_clip_image=None, num_images_per_prompt=1, image_scale=1.0,
                  num_samples=1, eta: float = 0.0, generator=None, output_type: Optional[str] = "pil",
@@ -399,17 +442,16 @@ class IMAGDressing_v1_ControlNet(_DressingPipelineBase):
                  controlnet_conditioning_scale: Union[float, List[float]] = 1.0, guess_mode: bool = False,
                  control_guidance_start=0.0, control_guidance_end=1.0, latents=None, garment_tokens=None,
                  ref_image_latents=None, adapter_image=None, adapter_conditioning_scale: float = 1.0, **kwargs):
-        start, end = _control_window(guess_mode, control_guidance_start, control_guidance_end)
+        ctrl, cscale, start, end = self._control_inputs(guess_mode, pose_image, controlnet_conditioning_scale,
+                                                        control_guidance_start, control_guidance_end, width, height)
         self.set_scale(image_scale)
-        ctrl = self.prepare_image(pose_image, width, height, self._execution_device) if pose_image is not None else None
         return self._run(prompt=prompt, negative_prompt=negative_prompt, ref_image=ref_image, width=width, height=height,
                          num_inference_steps=num_inference_steps, guidance_scale=guidance_scale,
                          ref_clip_image=ref_clip_image, num_images_per_prompt=num_images_per_prompt,
                          generator=generator, output_type=output_type, return_dict=return_dict, clip_skip=clip_skip,
                          callback=callback, prompt_embeds=prompt_embeds, negative_prompt_embeds=negative_prompt_embeds,
                          cross_attention_kwargs=cross_attention_kwargs, latents=latents, garment_tokens=garment_tokens,
-                         ref_image_latents=ref_image_latents, control_image=ctrl,
-                         controlnet_conditioning_scale=float(controlnet_conditioning_scale),
+                         ref_image_latents=ref_image_latents, control_image=ctrl, controlnet_conditioning_scale=cscale,
                          control_guidance_start=start, control_guidance_end=end, adapter_image=adapter_image,
                          adapter_conditioning_scale=adapter_conditioning_scale)
 
@@ -472,7 +514,8 @@ class IMAGDressing_v1_IPAControlNet(IMAGDressing_v1_ControlNet):
                  control_guidance_start=0.0, control_guidance_end=1.0, latents=None, garment_tokens=None,
                  ref_image_latents=None, face_clip_embeds=None, face_tokens=None, face_null_tokens=None,
                  adapter_image=None, adapter_conditioning_scale: float = 1.0, **kwargs):
-        start, end = _control_window(guess_mode, control_guidance_start, control_guidance_end)
+        ctrl, cscale, start, end = self._control_inputs(guess_mode, pose_image, controlnet_conditioning_scale,
+                                                        control_guidance_start, control_guidance_end, width, height)
         has_face = faceid_embeds is not None or face_tokens is not None
         if has_face:  # :433-438
             self.set_scale(image_scale, lora_scale=s_lora_scale)
@@ -482,7 +525,6 @@ class IMAGDressing_v1_IPAControlNet(IMAGDressing_v1_ControlNet):
         else:
             self.set_scale(image_scale, lora_scale=0.0)
             self.set_ipa_scale(0.0, 0.0)
-        ctrl = self.prepare_image(pose_image, width, height, self._execution_device) if pose_image is not None else None
         return self._run(prompt=prompt, negative_prompt=negative_prompt, ref_image=ref_image, width=width, height=height,
                          num_inference_steps=num_inference_steps, guidance_scale=guidance_scale,
                          ref_clip_image=ref_clip_image, num_images_per_prompt=num_images_per_prompt,
@@ -490,7 +532,7 @@ class IMAGDressing_v1_IPAControlNet(IMAGDressing_v1_ControlNet):
                          callback=callback, prompt_embeds=prompt_embeds, negative_prompt_embeds=negative_prompt_embeds,
                          cross_attention_kwargs=cross_attention_kwargs, latents=latents, garment_tokens=garment_tokens,
                          ref_image_latents=ref_image_latents, control_image=ctrl,
-                         controlnet_conditioning_scale=float(controlnet_conditioning_scale), face_tokens=face_tokens,
+                         controlnet_conditioning_scale=cscale, face_tokens=face_tokens,
                          face_null_tokens=face_null_tokens, control_guidance_start=start, control_guidance_end=end,
                          adapter_image=adapter_image, adapter_conditioning_scale=adapter_conditioning_scale)
 
@@ -511,10 +553,10 @@ class IMAGDressing_v1_ControlNetInpaint(IMAGDressing_v1_ControlNet):
                  guess_mode: bool = False, control_guidance_start=0.0, control_guidance_end=1.0, clip_skip=None,
                  garment_tokens=None, ref_image_latents=None, image_latents=None, mask_latents=None, adapter_image=None,
                  adapter_conditioning_scale: float = 1.0, **kwargs):
-        cg_start, cg_end = _control_window(guess_mode, control_guidance_start, control_guidance_end)
+        ctrl, cscale, cg_start, cg_end = self._control_inputs(guess_mode, control_image, controlnet_conditioning_scale,
+                                                              control_guidance_start, control_guidance_end, width, height)
         dev = self._execution_device
         self.set_scale(image_scale)
-        ctrl = self.prepare_image(control_image, width, height, dev) if control_image is not None else None
         if image_latents is None:
             if self.vae is None:
                 raise ValueError("no vae: pass image_latents and mask_latents")
@@ -533,9 +575,10 @@ class IMAGDressing_v1_ControlNetInpaint(IMAGDressing_v1_ControlNet):
             m = _image_batch(mask_image, w * self.vae_scale_factor, h * self.vae_scale_factor, gray=True)
             m = (m >= 0.5).to(device=dev, dtype=torch.float32)
             mask_latents = torch.nn.functional.interpolate(m, size=(h, w))
-        if ctrl is not None and tuple(ctrl.shape[-2:]) != (h * self.vae_scale_factor, w * self.vae_scale_factor):
-            raise ValueError(f"control_image {tuple(ctrl.shape[-2:])} does not match the image "
-                             f"{(h * self.vae_scale_factor, w * self.vae_scale_factor)}")
+        for c in (ctrl if isinstance(ctrl, list) else [ctrl] if ctrl is not None else []):
+            if tuple(c.shape[-2:]) != (h * self.vae_scale_factor, w * self.vae_scale_factor):
+                raise ValueError(f"control_image {tuple(c.shape[-2:])} does not match the image "
+                                 f"{(h * self.vae_scale_factor, w * self.vae_scale_factor)}")
         if mask_latents.shape[0] != n:
             mask_latents = mask_latents.expand(n, -1, -1, -1)
         noise = randn_tensor(image_latents.shape, generator=generator, device=dev) if latents is None else latents.to(dev)
@@ -556,7 +599,7 @@ class IMAGDressing_v1_ControlNetInpaint(IMAGDressing_v1_ControlNet):
                          callback=callback, prompt_embeds=prompt_embeds, negative_prompt_embeds=negative_prompt_embeds,
                          cross_attention_kwargs=cross_attention_kwargs, latents=start, garment_tokens=garment_tokens,
                          ref_image_latents=ref_image_latents, control_image=ctrl,
-                         controlnet_conditioning_scale=float(controlnet_conditioning_scale), mask=mask_latents,
+                         controlnet_conditioning_scale=cscale, mask=mask_latents,
                          image_latents=image_latents, strength=strength, noise=noise, control_guidance_start=cg_start,
                          control_guidance_end=cg_end, latents_scaled=True, adapter_image=adapter_image,
                          adapter_conditioning_scale=adapter_conditioning_scale)

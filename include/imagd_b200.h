@@ -66,6 +66,17 @@ typedef struct imagd_epilogue {
     int32_t ln_dim;             /* C of the folded LayerNorm (= K of this GEMM) */
     float ln_eps;
     const float* colsum;        /* consumer: [N] fp32 */
+    /* ---- per-step scale (the ControlNet zero convs of a multi-ControlNet step). When scale_table is non-NULL the kernel
+     * reads s = scale_table[scale_step[0] * scale_ld] on the device (row 0 when scale_step is NULL) and computes
+     *   out[r, c] = s * acc[r, c] + s * bias[c] + residual[r, c]
+     * with s * bias[c] rounded to fp32 on its own; alpha is ignored. For the same s this is bitwise the launch with
+     * alpha = s and bias = fp32(s * bias). A captured CUDA graph replays with whatever the table holds, and walks its
+     * rows as the step counter advances. imagd_gemm_bf16 only, with a plain bf16 epilogue: an activation, a row vector,
+     * a LayerNorm fold (either side), row statistics or an fp32 output is rejected, and so is a table passed to
+     * imagd_conv3x3_bf16 / imagd_upconv3x3_bf16 (IMAGD_ERR_ARG). Zero-initialise all three when unused. */
+    const float* scale_table;   /* fp32, 4-byte aligned; column k of an [S, K] table: base + k, scale_ld = K */
+    const int32_t* scale_step;  /* device step counter (the sampler's step_ptr) or NULL */
+    int64_t scale_ld;           /* row stride in floats, > 0 */
 } imagd_epilogue;
 
 /* D[M,N] = A[M,K] * W[N,K]^T (+ epilogue).  wgmma tensor cores, TMA-fed, fp32 accumulation.
